@@ -7,12 +7,19 @@
 Workload (config.workload): Mistral-7B FP16 single-stream decode (BASELINE.json configs[1]): 32 layers x
 7 bucketMul GEMVs (4096->4096 x2, 4096->1024 x2, 4096->14336 x2, 14336->4096) + rmsnorm / rope / attention /
 silu / residual + the dense 4096->32000 lm_head, random-initialised weights (no checkpoints offline), one
-token per step, greedy self-feeding.  A step = one token.  value = tokens/s at --effort (default 0.25, the
+token per step from a fixed seeded token sequence.  A step = one token.  value = tokens/s at --effort (default 0.25, the
 north-star operating point); the same run also reports effort 1.0 and 0.5 in `efforts`.
 
 Timing: W warm-up tokens (>= 3), then exactly K tokens between CUDA events on the launching stream with a
 barrier + synchronize on both sides, max over ranks.  Every token streams the selected rows of 14 GB of
-distinct weights (>> 126 MB L2), so no L2 flush is needed between iterations (config.l2).
+distinct weights (>> 50 MB L2), so no L2 flush is needed between iterations (config.l2).
+
+--dump-outputs DIR writes what the timed decode hands its caller after the last timed step: the logits
+(DIR/logits.npy, float32 [vocab]) and the next token (DIR/next_token.npy, float64 [1]).  Weights and the first
+tokens are seeded, so runs with the same arguments decode the same inputs, and the default kernels sum in a fixed
+order, so they compute the same bits.  Two different builds that sum in different orders still drift apart at low
+effort (rows move across the cutoff and the change grows through the 32 layers): compare their dumps with a tolerance
+that fits the effort.
 
 Besides the contract keys the line carries (rank 0, N = 1; each can be switched off, none touches the timed region):
   quality   per-token logit cos-sim of the effort-e decode against a DENSE decode of the same tokens (every projection
@@ -45,7 +52,7 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not a measured peak"
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -149,7 +156,7 @@ def workload_config(args, world):
                 f"tp{world}: q/k/v/w1/w3 column-sharded, wo/w2 row-sharded; per row-parallel GEMV one all-gather (cutoff "
                 f"input) + one all-reduce as one-shot NVLink peer-memory kernels fused with silu*mul / residual+rmsNorm "
                 f"(EFFORT_P2P=0: NCCL), vocab-sharded lm_head"),
-            "l2": "14 GB of distinct weights per token >> 126 MB L2: no flush needed"}
+            "l2": "14 GB of distinct weights per token >> 50 MB L2: no flush needed"}
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -286,17 +293,23 @@ def run_ours(args, rank, local_rank, world):
             torch.cuda.synchronize()
 
         def decode_device(effort, n_warm, n_steps):
+            # tokens from a fixed seeded sequence rather than the model's own argmax: every step then decodes the same
+            # input in every run and build (one argmax flipped by fp32 reordering would change all later inputs); a
+            # step copies its token on the device either way
+            n_warm = max(3, n_warm)
+            toks = torch.randint(0, cfg.vocab, (n_warm + n_steps,), generator=torch.Generator().manual_seed(4242),
+                                 dtype=torch.int32).cuda()
+            toks[0] = 1
+            toks = [toks[i:i + 1] for i in range(n_warm + n_steps)]
             model.reset()
-            tok = torch.tensor([1], dtype=torch.int32, device="cuda")
-            model.step(tok, effort)
-            for _ in range(max(3, n_warm) - 1):
-                model.step(None, effort)
+            for tok in toks[:n_warm]:
+                model.step(tok, effort)
             barrier()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             l0 = ops.launchCount()
             e0.record(stream)
-            for _ in range(n_steps):
-                model.step(None, effort)
+            for tok in toks[n_warm:]:
+                model.step(tok, effort)
             e1.record(stream)
             barrier()
             ms = e0.elapsed_time(e1)
@@ -306,6 +319,11 @@ def run_ours(args, rank, local_rank, world):
         with ClockSampler(index=local_rank, period=0.02) as cs:
             ms, launches = decode_device(args.effort, args.warmup, args.steps)
         clocks = cs.summary()
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "logits.npy"), model.logits().cpu().numpy().astype(np.float32))
+            np.save(os.path.join(args.dump_outputs, "next_token.npy"), np.array([model.next_token()], np.float64))
         t = torch.tensor([ms], dtype=torch.float64, device="cuda")
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -407,15 +425,7 @@ def run_ours(args, rank, local_rank, world):
             us = e0.elapsed_time(e1) * 1e3 / (reps * len(w1s))
             alg = args.effort * r_in * r_out * 2
             ach = alg / us / 1e3
-            traffic, traffic_src = None, None
-            try:  # dram__bytes_read+write per launch of the kernel from the committed ncu --set full capture (not re-measured here)
-                tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-                traffic = tr.get(str(args.effort)) if world == 1 else None
-                traffic_src = tr.get("source")
-            except Exception:
-                pass
-            roof = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
-                    "traffic_source": traffic_src,
+            roof = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                     "kernel": f"bucketMul {r_in}->{r_out}: one launch of the fused round-2 kernel (cutoff + selection + TMA-staged "
                               f"gather-MAC + reductions into out)",
                     "us_per_launch": us, "algorithmic_bytes": alg, "peak_source": peak_src}
@@ -541,7 +551,8 @@ def run_ours(args, rank, local_rank, world):
                 "data": "synthetic", "config": workload_config(args, world),
                 "e2e": {"value": e2e_tok_s, "unit": "tok/s", "h2d_bytes_per_step": 4, "d2h_bytes_per_step": 4 + 4 * cfg.vocab},
                 "gpu_launches": int(launches),
-                "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"]},
+                "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"],
+                           "gpu": clocks["gpu"], "power_limit_w": clocks["power_limit_w"]},
                 "roofline": roof, "cpu_baseline": cpu, "efforts": extras,
                 "token_roofline": {"bytes_per_token": bytes_tok, "tok_s_at_peak": roof_tok_s,
                                    "frac": (tok_s / streams_total) / roof_tok_s},
@@ -565,6 +576,7 @@ def main():
     ap.add_argument("--no-quality", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the heavy-tail quality, q4 and sweep records")
     ap.add_argument("--replicas", action="store_true", help="N>1: independent replicas instead of tensor parallelism")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's logits and next token as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,4 +1,4 @@
-"""effort_b200 -- B200-native implementation of kolinko/effort's bucketMul hot path.
+"""effort_b200 -- H100-native (sm_90a) implementation of kolinko/effort's bucketMul hot path.
 
 Only what the path needs lives here: csrc/ (CUDA kernels + the C-ABI of include/effort_b200.h) and the
 host-side mirror of the reference's operator interface (ops.py).  Importing the package does not touch

@@ -4,7 +4,7 @@
 // bucketMul (:83-117), bucketIntegrate (:122-137); Q4: prepareDispatchQ4 / bucketMulQ4
 // (bucketMulQ4.metal:25-92).
 //
-// B200 design (see DESIGN.md section 3):
+// Design (see DESIGN.md section 3):
 //  * HBM-bound gather, no tensor cores.  A bucket row is C 16-bit words; word (row r, column c) adds
 //    val_r * w into out[c*SLOTS + slot(w)] where slot is data dependent (4 position bits in the FP16
 //    mantissa; sign|pos nibbles in Q4).  The reference resolves the scatter with 16 predicated adds per

@@ -65,6 +65,9 @@ struct V2Problem {
     int* rounds_out;         // optional: CTA 0 stores the number of select rounds it needed
     unsigned* err_flag;      // set when the overwrite barrier times out
     unsigned long long* trace;
+    float4* red_part;        // bucket_mul_v4: [grid][kV2Threads] per-CTA partial sums of the epilogue
+    unsigned* red_sync;      // bucket_mul_v4: [CS][2] arrive / depart counters of the partial-sum exchange (zero between launches)
+    unsigned long long* unit_trace;  // bucket_mul_v4's unit / prologue stamps of CTA 0: the 712 words after the per-CTA rows
     float norm_eps;
     int in, C, P, q, layout, out_mode;
     int CS, RS, W;           // column slices, row splits, columns per slice (W = 32 * VEC except when C is smaller)
@@ -79,7 +82,7 @@ struct V2Batch {
     int prefetch;            // bucket_mul_v4_kernel: speculative L2 prefetch of the rows the hint selects
     int lookahead;           // bucket_mul_v4_kernel: consumers test the next unit's barrier / fetch its descriptor early
     int trace_cycles;        // EFFORT_TRACE=2: only the cheap SM-cycle stamps (the global-timer stamps perturb the phases)
-    int window;              // bucket_mul_v4_kernel (bulk): most units a producer takes per ticket grab (1..8)
+    int window;              // bucket_mul_v4_kernel (bulk): most units a producer issues per window (1..8)
     int cta_begin[kMulBatchMax + 1];
     V2Problem p[kMulBatchMax];
 };

@@ -11,8 +11,9 @@
 //    the next slot's barrier is tested and its descriptor fetched;
 //  * 8 PRODUCER warps (8-15), one per consumer.  Units are whole inputs: thread j of the CTA turns input j's selection
 //    mask into record j of a direct-indexed list {first 16-byte piece, rows, multiplier} (slice-major layout: the ranks an
-//    input selects inside this CTA's column slice are contiguous).  BULK (default): a producer takes a WINDOW of records
-//    from a shared ticket counter (guided sizes; work stealing between the pairs), hands out the pair's ring space by
+//    input selects inside this CTA's column slice are contiguous).  Each pair owns a fixed 1/8 of the pass's selected rows
+//    in list order, so the same rows reach the same tile in the same order in every run.  BULK (default): a producer
+//    takes WINDOWS of its range (ramped sizes), hands out the pair's ring space by
 //    shuffles, tests all outstanding slots' barriers in parallel and lets every lane issue its own unit: descriptor +
 //    mbarrier.arrive.expect_tx + ONE cp.async.bulk of 256..4096 bytes.  !BULK: one unit per step, copied with 16-byte
 //    cp.async by all lanes, completion through cp.async.mbarrier.arrive.noinc.  The slot comes back through a second
@@ -47,7 +48,8 @@ struct V4Header {
     float red[kV4SelWarps];
     float cutoff, denom;
     int sel_rows;
-    unsigned ticket;                     // next unit of the list a producer may take
+    uint32_t warp_rows[kV2Threads / 32]; // rows selected by each warp's records (the split below)
+    uint32_t start[kV4Pairs + 1];        // start[q]: the record holding pair q's first row (start[kV4Pairs] = records)
     unsigned long long full_bar[kV4Pairs][kV4Units];
     unsigned long long empty_bar[kV4Pairs][kV4Units];
     V4Desc desc[kV4Pairs][kV4Units];
@@ -182,7 +184,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     p += (size_t)NC * V4Smem::kTileBytes;
     V4Header& hdr = *reinterpret_cast<V4Header*>(p);
     p += V4Smem::kHdrBytes;
-    uint4* ulist = reinterpret_cast<uint4*>(p);  // the pass's units: {first 16-byte piece, rows, multiplier bits, -}
+    uint4* ulist = reinterpret_cast<uint4*>(p);  // the pass's units: {first 16-byte piece, rows, multiplier bits, rows before}
     p += (size_t)kV2MaxInputs * 16;
     p = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(p) + 127) & ~uintptr_t(127));
     float* ring_f = reinterpret_cast<float*>(p);
@@ -193,7 +195,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     const uint32_t e_no = pb.exp_no ? *pb.exp_no : 0u;
     V2_TRACE(0);
     // EFFORT_TRACE: SM-cycle stamps of the prologue phases of CTA 0, thread 0 (cheap, unlike the global timer)
-    unsigned long long* cst = (pb.trace && blockIdx.x == 0 && tid == 0) ? pb.trace + (size_t)kNumSMs * 16 + 696 : nullptr;
+    unsigned long long* cst = (pb.unit_trace && blockIdx.x == 0 && tid == 0) ? pb.unit_trace + 696 : nullptr;
     if (cst) cst[0] = (unsigned long long)clock64();
 
     // ---- 0. constant metadata before the dependency wait ----
@@ -239,7 +241,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
             mbar_init((uint32_t)__cvta_generic_to_shared(&hdr.full_bar[0][0] + s), BULK ? 1 : 33);
             mbar_init((uint32_t)__cvta_generic_to_shared(&hdr.empty_bar[0][0] + s), 1);
         }
-        if (lane == 0) { hdr.ticket = 0u; hdr.sel_rows = 0; }
+        if (lane == 0) hdr.sel_rows = 0;
         // (the __syncthreads before the first use orders the initialisation: no cluster, no async-proxy user here)
     }
     // Everything the streaming phase needs that does not depend on the input vector is set up HERE, before the dependency
@@ -258,13 +260,12 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     const uint32_t my_src0 = src_of(tid);
 
     // debugging aid (EFFORT_TRACE): issue / arrival / release times of the first 80 units of pair 0 of CTA 0
-    unsigned long long* utrace = (pb.trace && blockIdx.x == 0 && pair == 0) ? pb.trace + (size_t)kNumSMs * 16 : nullptr;
+    unsigned long long* utrace = (pb.unit_trace && blockIdx.x == 0 && pair == 0) ? pb.unit_trace : nullptr;
     if (utrace && tid == 0) utrace[640] = (unsigned long long)clock64();  // time base: the SM's cycle counter
     // pair state.  Both sides count units (seq); unit s uses descriptor slot s % kV4Units, barrier phase (s / kV4Units) & 1.
     // Producer only: ring head, free bytes, oldest unit not yet reclaimed.
     uint32_t seq = 0, tail_seq = 0, head = 0, free_b = kV4RingBytes;
     uint32_t slot_charged = 0u;  // bulk producers: lane s remembers the ring bytes the unit in descriptor slot s holds
-    const uint32_t ticket_saddr = (uint32_t)__cvta_generic_to_shared(&hdr.ticket);
     const uint32_t full0 = (uint32_t)__cvta_generic_to_shared(&hdr.full_bar[pair][0]);
     const uint32_t empty0 = (uint32_t)__cvta_generic_to_shared(&hdr.empty_bar[pair][0]);
     const uint32_t desc0 = (uint32_t)__cvta_generic_to_shared(&hdr.desc[pair][0]);
@@ -438,7 +439,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     V2_TRACE(6);
 
     if (cst) cst[11] = (unsigned long long)clock64();
-    bool pristine = true;  // the ticket counter still at its initial zero
+    bool pristine = true;  // no earlier round has used the unit list
     // ---- passes over the inputs of this row split (one pass for every Mistral shape) ----
     for (int j0 = 0; j0 < n_in; j0 += NT) {
         const int j = j0 + tid;
@@ -476,16 +477,14 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
         // take one round per run. ----
         bool more;
         do {
-            if (!pristine) {
-                __syncthreads();
-                if (tid == 0) hdr.ticket = 0u;
-                __syncthreads();
-            }
+            if (!pristine) __syncthreads();  // the producers are done with the previous round's list
             pristine = false;
+            const uint32_t nu_pass = (uint32_t)min(NT, n_in - j0);  // records of this pass (empty ones included)
+            uint32_t len = 0u;
             if (warp_has_inputs) {
                 // 2b. the unit list: record j of the pass belongs to input j -- no compaction, no atomics on this serial stretch;
                 // an input that selects nothing leaves an empty record (rows = 0) that the producers skip
-                uint32_t st = 0u, len = 0u;
+                uint32_t st = 0u;
                 if (m) {
                     st = (uint32_t)__ffs((int)m) - 1u;
                     len = (uint32_t)__ffs((int)~(m >> st)) - 1u;
@@ -494,18 +493,60 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                 ulist[tid] = make_uint4(my_src + st * rs16, len, __float_as_uint(my_val), 0u);
             }
             if (cst && j0 == 0) cst[6] = (unsigned long long)clock64();
+            // rows up to and including this record inside its warp; the warp totals go to the header
+            uint32_t incl = len;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += y;
+            }
+            if (lane == 31) hdr.warp_rows[warp] = incl;
+            if (tid <= NC) hdr.start[tid] = tid ? nu_pass : 0u;
             more = __syncthreads_or(m != 0u) != 0;
+            // 2c. pair q accumulates rows [floor(q * total / NC), floor((q + 1) * total / NC)) of the pass in list order; a record
+            // that straddles a boundary is cut between two pairs.  A static split, exact in rows, that fixes which tile
+            // accumulates which row: the sums do not depend on timing.  start[q] = the record holding the pair's first row.
+            uint32_t row_lo, row_hi;
+            {
+                uint32_t off = 0u, total = 0u;
+#pragma unroll
+                for (int w = 0; w < NT / 32; w++) {
+                    const uint32_t x = hdr.warp_rows[w];
+                    total += x;
+                    if (w < warp) off += x;
+                }
+                row_lo = (uint32_t)pair * total / NC;
+                row_hi = (uint32_t)(pair + 1) * total / NC;
+                if ((uint32_t)tid < nu_pass) {
+                    const uint32_t e = off + incl - len;  // rows of the records before this one
+                    ulist[tid].w = e;
+#pragma unroll
+                    for (int q = 1; q < NC; q++) {
+                        const uint32_t T = (uint32_t)q * total / NC;
+                        if (e <= T && T < e + len) hdr.start[q] = (uint32_t)tid;
+                    }
+                }
+                __syncthreads();
+            }
+            // this pair's part of record `rec`: rows [row_lo, row_hi) of the pass
+            auto clip = [&](uint4 rec) {
+                const uint32_t lo = max(rec.w, row_lo), hi = min(rec.w + rec.y, row_hi);
+                rec.x += (lo - rec.w) * rs16;
+                rec.y = hi > lo ? hi - lo : 0u;
+                return rec;
+            };
+            const uint32_t r_next = hdr.start[pair + 1];
+            const uint32_t r_end = r_next < nu_pass ? r_next + 1u : nu_pass;  // (the record holding the next pair's first row)
             if (cst && j0 == 0) cst[7] = (unsigned long long)clock64();
             V2_TRACE(8);
 
             if (!consumer && BULK) {
-                // ---- 3a. producer of pair `pair`, bulk copies.  Every shared-memory operation of a producer (ticket, record,
+                // ---- 3a. producer of pair `pair`, bulk copies.  Every shared-memory operation of a producer (record,
                 // barrier test, descriptor) queues behind the consumers' read-modify-writes -- the shared-memory pipe is the
                 // kernel's bottleneck (tools/ubench/stage_cost.cu: ~350 cycles per dependent operation) -- so a producer works
-                // on a WINDOW of units at once, one per lane: one ticket grab (guided: remaining/16, 1..8 units), the records in
+                // on a WINDOW of units of its range at once, one per lane (1..8 units, ramped up), the records in
                 // parallel, ring space handed out by shuffles, the barrier tests of all outstanding slots in parallel, and each
                 // lane issues its own unit's descriptor + expect_tx + bulk copy. ----
-                const uint32_t nu = (uint32_t)min(NT, n_in - j0);  // records of this pass (empty ones included)
                 auto reclaim = [&](bool block) {  // take back the bytes of every unit the consumer has released (in order)
                     const uint32_t out_n = seq - tail_seq;
                     const uint32_t rel = ((uint32_t)lane - tail_seq) & (kV4Units - 1);  // slot `lane`: distance from the oldest
@@ -527,21 +568,14 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                     free_b += got;
                     tail_seq += n;
                 };
-                uint32_t t_seen = 0u, grabs = 0u;
+                uint32_t t0 = hdr.start[pair], grabs = 0u;
 #pragma unroll 1
-                for (;;) {
-                    const uint32_t left = nu > t_seen ? nu - t_seen : 0u;
-                    // guided grabs, ramped up: the very first units of all pairs must not queue behind a burst
-                    const uint32_t want = min(min((uint32_t)batch.window, 1u + grabs), max(1u, left / (2u * NC)));
+                for (; t0 < r_end; t0 += min(min((uint32_t)batch.window, grabs), r_end - t0)) {
+                    // windows ramped up: the very first units must not queue behind a burst
                     grabs++;
-                    uint32_t t0 = 0u;
-                    if (lane == 0) asm volatile("atom.shared.add.u32 %0, [%1], %2;" : "=r"(t0) : "r"(ticket_saddr), "r"(want) : "memory");
-                    t0 = __shfl_sync(0xffffffffu, t0, 0);
-                    if (t0 >= nu) break;
-                    t_seen = t0 + want;
-                    const uint32_t cnt = min(want, nu - t0);
+                    const uint32_t cnt = min(min((uint32_t)batch.window, grabs), r_end - t0);
                     uint4 rec = make_uint4(0u, 0u, 0u, 0u);
-                    if ((uint32_t)lane < cnt) rec = ulist[t0 + lane];
+                    if ((uint32_t)lane < cnt) rec = clip(ulist[t0 + lane]);
                     const uint32_t my_bytes = rec.y * (uint32_t)seg_bytes;
                     uint32_t pos = 0u;
                     if (seq != tail_seq) reclaim(false);
@@ -594,12 +628,6 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                 }
             } else if (!consumer) {
                 // ---- 3a'. producer of pair `pair`, 16-byte cp.async by all lanes, one unit at a time ----
-                const uint32_t nu = (uint32_t)min(NT, n_in - j0);
-                auto grab = [&]() {
-                    uint32_t t = 0u;
-                    if (lane == 0) asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(t) : "r"(ticket_saddr) : "memory");
-                    return t;
-                };
                 auto reclaim = [&]() {  // wait for the consumer to release the oldest unit, take its bytes back
                     const uint32_t ts = tail_seq & (kV4Units - 1);
                     if (!mbar_wait_parked(empty0 + ts * 8u, (tail_seq / kV4Units) & 1u)) {
@@ -633,13 +661,9 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                     free_b -= bytes + skip;
                     if (head >= (uint32_t)kV4RingBytes) head = 0u;
                 };
-                uint32_t tk = grab();
 #pragma unroll 1
-                for (;;) {
-                    const uint32_t t = __shfl_sync(0xffffffffu, tk, 0);
-                    if (t >= nu) break;
-                    const uint4 rec = ulist[t];
-                    tk = grab();  // the next ticket travels while this unit is issued
+                for (uint32_t t = hdr.start[pair]; t < r_end; t++) {
+                    const uint4 rec = clip(ulist[t]);
                     if (rec.y != 0u) fill(rec.x, rec.y, rec.z);  // (an input that selected nothing left an empty record)
                 }
                 fill(0u, 0u, 0u);  // stop marker for the consumer
@@ -711,8 +735,8 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                     if (utrace && lane == 0 && seq <= 80u) utrace[8 * (seq - 1) + 7] = (unsigned long long)clock64();
                 }
                 if (lane == 0 && rows_done) atomicAdd(&hdr.sel_rows, (int)rows_done);  // rows selected = rows accumulated
-                if (pb.trace && blockIdx.x == 0 && lane == 0) {  // when every consumer of CTA 0 ran dry, and how much it did
-                    unsigned long long* fin = pb.trace + (size_t)kNumSMs * 16 + 648;
+                if (pb.unit_trace && blockIdx.x == 0 && lane == 0) {  // when every consumer of CTA 0 ran dry, and how much it did
+                    unsigned long long* fin = pb.unit_trace + 648;
                     fin[warp] = (unsigned long long)clock64();
                     fin[16 + warp] = rows_done;
                     fin[32 + warp] = (unsigned long long)seq;
@@ -725,7 +749,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     V2_TRACE(9);
     if (cst) cst[8] = (unsigned long long)clock64();
 
-    // ---- 4. CTA epilogue: sum the 8 consumer tiles and add into out ----
+    // ---- 4. CTA epilogue: sum the 8 consumer tiles; the RS partial sums of the slice then meet in a fixed order ----
     {
         constexpr int NG = NT / TW, SPT = SLOTS / NG;
         static_assert(SPT == 4, "one 16-byte reduction per thread");
@@ -742,10 +766,24 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                     for (int s = 0; s < SPT; s++) acc[s] += tiles[(size_t)w * TF + word0 + s * TW];
             }
         }
-        if (pb.out_mode == kOutOverwrite) {
-            if (tid == 0) {
+        // this CTA's partial sum goes to scratch; once all RS CTAs of the slice have written theirs, CTA rsp adds positions
+        // rsp, rsp + RS, ... of the slice, each the sum over the RS partials in row-split order: every output word gets ONE
+        // addition per launch, so the result does not depend on which CTA finished first
+        pb.red_part[(size_t)blockIdx.x * NT + tid] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        __threadfence();
+        __syncthreads();
+        unsigned* rsy = pb.red_sync + 2 * slice;
+        if (tid == 0) {
+            atomicAdd(rsy, 1u);
+            const unsigned long long t0 = gtime_ns();
+            while (ld_acquire_u32(rsy) < (unsigned)RS) {
+                if (gtime_ns() - t0 > 2000000000ull) {
+                    if (pb.err_flag) atomicExch(pb.err_flag, 4u);
+                    break;
+                }
+            }
+            if (pb.out_mode == kOutOverwrite) {
                 const unsigned* cnt = pb.sync + 2 * slice;
-                const unsigned long long t0 = gtime_ns();
                 while (ld_acquire_u32(cnt) < (unsigned)RS) {
                     if (gtime_ns() - t0 > 2000000000ull) {
                         if (pb.err_flag) atomicExch(pb.err_flag, 1u);
@@ -753,18 +791,30 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                     }
                 }
             }
-            __syncthreads();
         }
-        if (col_on) {
-            const int col = slice * pb.W + ln * VEC + k;
-            red_add_v4(pb.out + (size_t)col * SLOTS + sg * SPT, acc[0], acc[1], acc[2], acc[3]);
+        __syncthreads();
+        const int t = rsp + tid * RS;
+        if (t < NT) {
+            const int tcl = t % TW, tsg = t / TW, tk = tcl >> 5, tln = tcl & 31;
+            if ((tln < lpr) && (tln * VEC + tk < slice_cols)) {
+                const float4* src = pb.red_part + (size_t)(batch.cta_begin[pi] + slice) * NT + t;
+                float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int r = 0; r < RS; r++) {
+                    const float4 x = __ldcg(src + (size_t)r * pb.CS * NT);
+                    sum.x += x.x; sum.y += x.y; sum.z += x.z; sum.w += x.w;
+                }
+                const int col = slice * pb.W + tln * VEC + tk;
+                red_add_v4(pb.out + (size_t)col * SLOTS + tsg * SPT, sum.x, sum.y, sum.z, sum.w);
+            }
         }
-        if (pb.out_mode == kOutOverwrite) {
-            __syncthreads();
-            if (tid == 0) {
+        __syncthreads();
+        if (tid == 0) {
+            const unsigned old = atomicAdd(rsy + 1, 1u);
+            if (old == (unsigned)RS - 1u) { rsy[0] = 0u; rsy[1] = 0u; }
+            if (pb.out_mode == kOutOverwrite) {
                 unsigned* sy = pb.sync + 2 * slice;
-                const unsigned old = atomicAdd(sy + 1, 1u);
-                if (old == (unsigned)RS - 1u) { sy[0] = 0u; sy[1] = 0u; }
+                const unsigned o2 = atomicAdd(sy + 1, 1u);
+                if (o2 == (unsigned)RS - 1u) { sy[0] = 0u; sy[1] = 0u; }
             }
         }
     }

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the effort_b200 kernels (sm_100a only).
+// common.cuh -- shared device helpers for the effort_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -8,7 +8,6 @@
 namespace effort {
 
 constexpr float kCutoffScale = 100000.0f;  // CUTOFF_SCALE, bucketMul.metal:33
-constexpr int kNumSMs = 148;               // B200
 
 // fp32 -> bfloat16 -> fp32, round-to-nearest-even; integer form so that it is bit-identical to the
 // oracle (Metal `bfloat(x)`, bucketMul.metal:160).

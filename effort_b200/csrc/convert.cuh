@@ -1,7 +1,7 @@
 // convert.cuh -- one-time weight conversion (reference: convert.swift:209-260 + convert.metal:14-119)
 // and the load-time device repack.
 //
-// B200-first restructuring of bucketize: the reference sorts every transposed weight row by |w|
+// GPU-first restructuring of bucketize: the reference sorts every transposed weight row by |w|
 // (in x log^2(out) bitonic launches, convert.swift:227-229) only to walk it and deal the weights into
 // their 16-wide buckets in arrival order.  The rank a weight gets inside its bucket depends only on
 // the 16 weights of that bucket, so one thread ranks one (input, bucket) group by counting -- a single

@@ -1,4 +1,4 @@
-// effort_capi.cu -- the C-ABI shim (include/effort_b200.h) over the sm_100a kernels.
+// effort_capi.cu -- the C-ABI shim (include/effort_b200.h) over the sm_90a kernels.
 // Host orchestration here mirrors bucketMul.swift:34-88 / bucketMulQ4.swift:35-85 / expertMul.swift:20-38.
 #include "../../include/effort_b200.h"
 
@@ -66,7 +66,7 @@ struct effort_weights {
 
 struct effort_ctx {
     int device = 0;
-    int n_sms = kNumSMs;
+    int n_sms = 0;               // multiProcessorCount of `device`
     // scratch
     float* cutoff = nullptr;     // [kMaxBatch]
     int* loops = nullptr;        // [1]
@@ -85,13 +85,15 @@ struct effort_ctx {
     // round-2 fused kernel (bucket_mul_v2.cuh)
     unsigned* v2_sync = nullptr;          // [kMaxBatch][kV2MaxSlices][2] arrive/depart counters (overwrite protocol)
     unsigned* v2_err = nullptr;           // [1] set by a kernel whose overwrite barrier timed out
+    float4* v4_part = nullptr;            // [n_sms][kV2Threads] bucket_mul_v4 epilogue partial sums
+    unsigned* v4_sync = nullptr;          // [kMaxBatch][kV2MaxSlices][2] bucket_mul_v4 partial-sum exchange counters
     int cutoff_mode = 0;                  // EFFORT_CUTOFF_SELECT / EFFORT_CUTOFF_BISECT
     int stage_mode = 4;                   // 4 = consumer/producer warp pairs fed by bulk copies (slice-major FP16 weights; default), 3 = the pairs with 16-byte cp.async
                                           // 2 = one TMA producer warp + byte ring (slice-major FP16 weights; measured slower)
                                           // 0 = per-warp cp.async rings, units of <= 4 rows (any layout, Q4)
     int engine = 2;                       // 2 = bucket_mul_v2_kernel, 1 = round-1 fused kernel + integrate
     int lookahead = 1;                    // bucket_mul_v4 consumers: test the next slot and fetch its descriptor while the current unit is accumulated
-    int window = 8;                       // bucket_mul_v4 bulk producers: most units per ticket grab
+    int window = 8;                       // bucket_mul_v4 bulk producers: most units per window
     int prefetch = 0;                     // bucket_mul_v4: speculative L2 prefetch of the rows the previous cutoff selects
                                           // (measured: no gain at effort 0.25, -13 % at 1.0: the gather is not DRAM-latency bound)
     int use_hint = 1;                     // bucket_mul_v4: the select starts from the matrix's previous cutoff
@@ -150,6 +152,9 @@ extern "C" int effort_ctx_create(int device, effort_ctx_t** ctx_out) {
     CK(cudaMemset(c->loops, 0, sizeof(int)));
     CK(cudaMalloc(&c->v2_sync, sizeof(unsigned) * kMaxBatch * kV2MaxSlices * 2));
     CK(cudaMemset(c->v2_sync, 0, sizeof(unsigned) * kMaxBatch * kV2MaxSlices * 2));
+    CK(cudaMalloc(&c->v4_part, sizeof(float4) * kV2Threads * c->n_sms));
+    CK(cudaMalloc(&c->v4_sync, sizeof(unsigned) * kMaxBatch * kV2MaxSlices * 2));
+    CK(cudaMemset(c->v4_sync, 0, sizeof(unsigned) * kMaxBatch * kV2MaxSlices * 2));
     CK(cudaMalloc(&c->v2_err, sizeof(unsigned)));
     CK(cudaMemset(c->v2_err, 0, sizeof(unsigned)));
     CK(cudaMalloc(&c->sel_counts, sizeof(uint32_t) * kMaxBatch * c->n_sms));  // fixed size: graphs keep the pointer
@@ -218,7 +223,7 @@ extern "C" int effort_ctx_destroy(effort_ctx_t* c) {
     if (!c) return EFFORT_OK;
     cudaFree(c->cutoff); cudaFree(c->loops); cudaFree(c->sizes); cudaFree(c->dispatch);
     cudaFree(c->chunk_counts); cudaFree(c->partial); cudaFree(c->sel_counts);
-    cudaFree(c->trace); cudaFree(c->v2_sync); cudaFree(c->v2_err);
+    cudaFree(c->trace); cudaFree(c->v2_sync); cudaFree(c->v2_err); cudaFree(c->v4_part); cudaFree(c->v4_sync);
     for (int p = 0; p < 16; p++)
         if (c->p2p_peer[p] && c->p2p_peer[p] != (void*)c->p2p_local) cudaIpcCloseMemHandle(c->p2p_peer[p]);
     cudaFree(c->p2p_local);
@@ -500,6 +505,9 @@ template <int SLOTS, int VEC>
 static int launch_v2_batch(effort_ctx* ctx, const V2Call* calls, int n, int slot0, cudaStream_t stream) {
     if (n < 1 || n > kMulBatchMax) return EFFORT_EINVAL;
     constexpr int D = 4;
+    // at most one CTA per SM (every variant needs most of the SM's shared memory), so all CTAs of a launch are resident
+    // at once: the in-kernel waits between the CTAs of a column slice rely on it (overwrite zeroing; bucket_mul_v4's
+    // partial-sum exchange)
     const int n_cta = ctx->n_sms;
     V2Batch batch{};
     batch.n = n;
@@ -532,12 +540,15 @@ static int launch_v2_batch(effort_ctx* ctx, const V2Call* calls, int n, int slot
         pb.st16 = w->st16; pb.st32 = w->st32; pb.bk = w->fast_bk(); pb.probes = w->probes; pb.exp_no = c.exp_no;
         pb.out = c.out; pb.out_scale = c.out_scale;
         pb.sync = ctx->v2_sync + (size_t)(slot0 + k) * kV2MaxSlices * 2;
+        pb.red_sync = ctx->v4_sync + (size_t)(slot0 + k) * kV2MaxSlices * 2;
+        pb.red_part = ctx->v4_part;
         pb.sel_counts = ctx->sel_counts + (size_t)(slot0 + k) * ctx->n_sms;
         pb.cutoff_out = ctx->cutoff + slot0 + k;
         pb.cutoff_hint = ctx->use_hint ? w->hint : nullptr;
         pb.rounds_out = (slot0 + k == 0) ? ctx->loops : nullptr;
         pb.err_flag = ctx->v2_err;
         pb.trace = ctx->trace;
+        pb.unit_trace = ctx->trace ? ctx->trace + 16 * ctx->n_sms : nullptr;
         pb.in = w->in; pb.C = w->C; pb.P = w->P; pb.q = effort_q(c.effort, w->n_probes); pb.layout = w->layout;
         pb.out_mode = c.out_mode;
         pb.CS = g.CS; pb.RS = rs; pb.W = (g.CS == 1) ? w->C : 32 * VEC; pb.R = g.R; pb.lpr = g.lpr;

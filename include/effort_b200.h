@@ -1,5 +1,5 @@
 /*
- * effort_b200.h -- C-ABI of the B200-native bucketMul hot path.
+ * effort_b200.h -- C-ABI of the H100-native (sm_90a) bucketMul hot path.
  *
  * Drop-in boundary for kolinko/effort's approximate GEMV.  The reference has no
  * FFI layer today: its boundary is a handful of Swift free functions plus the

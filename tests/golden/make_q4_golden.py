@@ -1,8 +1,8 @@
 """Generates tests/golden/q4_golden_*.npz by running the REFERENCE's own Q4 converter
-(/root/reference/q4_draft.py:70-322, function convert) on small seeded matrices.
+(q4_draft.py:70-322 of kolinko/effort, function convert) on small seeded matrices.
 
-Run in the build container only (the reference does not travel to the GPU box):
-    python tests/golden/make_q4_golden.py
+Needs a checkout of the reference; the tests read only the stored fixtures:
+    python tests/golden/make_q4_golden.py <path to the reference's q4_draft.py>
 q4_draft.convert reads a module-global `v` (q4_draft.py:209) that the reference never defines at
 module level, so it is injected before the call.  Nothing is copied from the reference: the
 fixtures hold only its INPUTS and OUTPUTS.
@@ -16,11 +16,8 @@ import sys
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/q4_draft.py"
-
-
-def load_ref():
-    spec = importlib.util.spec_from_file_location("q4_draft_ref", REF)
+def load_ref(path):
+    spec = importlib.util.spec_from_file_location("q4_draft_ref", path)
     mod = importlib.util.module_from_spec(spec)
     with contextlib.redirect_stdout(io.StringIO()):
         spec.loader.exec_module(mod)
@@ -28,7 +25,7 @@ def load_ref():
 
 
 def main():
-    ref = load_ref()
+    ref = load_ref(sys.argv[1])
     for name, inn, out, seed in [("a", 64, 64, 11), ("b", 96, 128, 12), ("c", 32, 256, 13)]:
         rng = np.random.default_rng(seed)
         core2 = (rng.standard_normal((inn, out)) * 0.02).astype(np.float16)  # W^T [in, out]

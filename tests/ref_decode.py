@@ -39,6 +39,8 @@ class RefModel:
 
     def _mul(self, v, w, effort, exp_no=0):
         if w.get("n_experts", 1) > 1:   # expNo selects the expert's rows / probes (bucketMul.metal:49,143)
+            if self.fast:
+                return O.bucket_mul_mt(v, w["buckets"], w["stats"], w["probes"], w["in"], w["out"], effort, exp_no=exp_no)[0]
             r = O.bucket_mul(v, w["buckets"], w["stats"], w["probes"], w["in"], w["out"], effort, exp_no=exp_no)
             return r["out32"]
         return self._mul1(v, w, effort)

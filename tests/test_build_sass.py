@@ -1,4 +1,4 @@
-"""Static checks on the compiled sm_100a code of the hot kernels (no GPU needed: cuobjdump reads the in-tree .so).
+"""Static checks on the compiled sm_90a code of the hot kernels (no GPU needed: cuobjdump reads the in-tree .so).
 They pin the properties DESIGN.md section 4 claims: no local-memory spills, the packed bf16 counting of the cutoff,
 non-allocating streaming loads, no tensor-core instructions on this HBM-bound path."""
 import re

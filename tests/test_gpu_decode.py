@@ -13,6 +13,27 @@ def _cpu(t):
     return t.cpu().numpy()
 
 
+def _restatements(layers, head):
+    """The CPU restatement in both of its summation forms: the sequential oracle (float64 sums) and its OpenMP port
+    (float32 sums, as on the device).  They alone can differ by more than the decode bars below: in bisect mode a
+    last-bit change of one layer's output moves the next layer's bisection cutoff, and the two forms drift to cos-sim
+    0.998 on the 2-layer model after one token.  A decoded token must match one of them within the bar.
+
+    Measured on an H100 (first token, the 2-layer model of `_small`): bisect mode (engines 1 and 2), GPU vs float64
+    oracle 0.998189, GPU vs float32 port 1.000000, oracle vs port 0.998189; select mode 1.000000 for all three.  The MoE
+    model against the float64 oracle alone: 0.99928 on its first token."""
+    return RefModel(layers, *head), RefModel(layers, *head, fast=True)
+
+
+def _reset(refs):
+    for r in refs:
+        r.pos, r.kc, r.vc = 0, [[] for _ in r.layers], [[] for _ in r.layers]
+
+
+def _cossim_best(got, refs, token, effort):
+    return max(O.cossim(got, r.step(token, effort)) for r in refs)
+
+
 def _small(flags):
     import torch
     from effort_b200 import ops
@@ -28,8 +49,7 @@ def _small(flags):
                     "out": ew.outSize}
         d["attn_norm"], d["ffn_norm"] = _cpu(L[7]), _cpu(L[8])
         layers.append(d)
-    ref = RefModel(layers, _cpu(m.head[0]), _cpu(m.head[1]), _cpu(m.head[2]))
-    return m, ref
+    return m, _restatements(layers, [_cpu(t) for t in m.head[:3]])
 
 
 @pytest.fixture(scope="module")
@@ -57,7 +77,7 @@ def _select_mode():
 def test_decode_matches_cpu_restatement(small_model, small_model_input_major, use_graph, chain, engine, fused_glue):
     import torch
     from effort_b200 import ops
-    m, ref = small_model_input_major if engine == 1 else small_model
+    m, refs = small_model_input_major if engine == 1 else small_model
     ctx = ops.default_context()
     try:
         ctx.setOption("engine", engine)
@@ -68,15 +88,14 @@ def test_decode_matches_cpu_restatement(small_model, small_model_input_major, us
         m.set_chain(chain)
         m.set_fused_glue(fused_glue)
         m.reset()
-        ref.pos, ref.kc, ref.vc = 0, [[] for _ in ref.layers], [[] for _ in ref.layers]
+        _reset(refs)
         toks = [1, 17, 400, 999, 5]
         for t in toks:
             tok = torch.tensor([t], dtype=torch.int32, device="cuda")
             m.step(tok, effort=0.5)
             torch.cuda.synchronize()
             got = m.logits().cpu().numpy()
-            want = ref.step(t, 0.5)
-            cs = O.cossim(got, want)
+            cs = _cossim_best(got, refs, t, 0.5)
             assert cs > 0.9995, cs     # tiny selection flips (fp32 reorder of v near the cutoff) allowed
             assert m.next_token() == int(np.argmax(got))
         assert ctx.errorFlag() == 0
@@ -198,7 +217,7 @@ def test_model_directory_roundtrip(tmp_path):
             torch.cuda.synchronize()
             seq.append(m.logits().cpu().numpy())
         outs[name] = seq
-    for name in ("native", "python"):   # same weights; the CTA sums meet in the outputs in no fixed order
+    for name in ("native", "python"):   # same weights in separately converted copies
         for a, b in zip(outs["mem"], outs[name]):
             assert O.cossim(a, b) > 0.999999, name
     # percentLoad 8 drops ranks 8..15.  On iid-Gaussian weights those ranks ARE selected at effort 0.25 (the row means
@@ -253,15 +272,14 @@ def test_moe_decode_matches_cpu_restatement():
                     "out": ew.outSize, "n_experts": ew.numExperts}
         d["attn_norm"], d["ffn_norm"], d["gate"] = _cpu(L[7]), _cpu(L[8]), _cpu(L[9])
         layers.append(d)
-    ref = RefModel(layers, _cpu(m.head[0]), _cpu(m.head[1]), _cpu(m.head[2]))
+    refs = _restatements(layers, [_cpu(t) for t in m.head[:3]])
     for use_graph in (False, True):
         m.set_graphs(use_graph)
         m.reset()
-        ref.pos, ref.kc, ref.vc = 0, [[] for _ in layers], [[] for _ in layers]
+        _reset(refs)
         for t in (1, 17, 400):
             m.step(torch.tensor([t], dtype=torch.int32, device="cuda"), effort=0.5)
             torch.cuda.synchronize()
             got = m.logits().cpu().numpy()
-            want = ref.step(t, 0.5)
-            assert O.cossim(got, want) > 0.9995
+            assert _cossim_best(got, refs, t, 0.5) > 0.9995
             assert m.next_token() == int(np.argmax(got))

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): every call goes through the C-ABI (effort_b200.ops -> ctypes ->
+"""GPU parity tests (run on an H100): every call goes through the C-ABI (effort_b200.ops -> ctypes ->
 libeffort_b200.so) and is checked against the CPU oracle on the same seeded inputs.
 
 Bars (SURVEY.md section 8c):

@@ -9,13 +9,16 @@ class ClockSampler:
         self.samples, self.reasons = [], set()
         self._stop = threading.Event()
         self._t = None
-        self.max_mhz = None
+        self.max_mhz = self.name = self.power_limit_w = None
         try:
             import pynvml
             pynvml.nvmlInit()
             self._nv = pynvml
             self._h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self._h, pynvml.NVML_CLOCK_SM)
+            name = pynvml.nvmlDeviceGetName(self._h)
+            self.name = name.decode() if isinstance(name, bytes) else name
+            self.power_limit_w = pynvml.nvmlDeviceGetPowerManagementLimit(self._h) / 1000.0   # mW -> W
         except Exception:
             self._nv = None
 
@@ -56,4 +59,5 @@ class ClockSampler:
     def summary(self):
         s = sorted(self.samples)
         med = s[len(s) // 2] if s else None
-        return {"sm_mhz": med, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(s)}
+        return {"sm_mhz": med, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(s),
+                "gpu": self.name, "power_limit_w": self.power_limit_w}

@@ -30,8 +30,9 @@ for rep in range(3):
     ops.bucketMul(v, ws[rep % 4], None, out, a.effort)
     e.record()
     torch.cuda.synchronize()
-    buf = np.zeros((148, 16), dtype=np.uint64)
-    n = L.effort_debug_read_trace(ctx._h, buf.ctypes.data, 148)
+    n_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    buf = np.zeros((n_sms, 16), dtype=np.uint64)
+    n = L.effort_debug_read_trace(ctx._h, buf.ctypes.data, n_sms)
     t = buf[:n, :11].astype(np.int64)
     loops = buf[:n, 11:13]
     sorted_t = buf[:n, 13].astype(np.int64)

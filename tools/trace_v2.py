@@ -34,8 +34,9 @@ for rep in range(3):
     ops.bucketMul(v, ws[rep % 4], None, out, a.effort)
     e.record()
     torch.cuda.synchronize()
-    buf = np.zeros((148, 16), dtype=np.uint64)
-    n = L.effort_debug_read_trace(ctx._h, buf.ctypes.data, 148)
+    n_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    buf = np.zeros((n_sms, 16), dtype=np.uint64)
+    n = L.effort_debug_read_trace(ctx._h, buf.ctypes.data, n_sms)
     t = buf[:n].astype(np.int64)
     t = t[t[:, 0] > 0]
     if len(t) == 0:          # EFFORT_TRACE=2: cycle stamps only

@@ -1,6 +1,6 @@
 // Micro-benchmark: how fast can W warps of ONE SM run the accumulate step of bucket_mul_v4_kernel when the staged rows
 // already sit in shared memory?  Separates the warp-level dependency chain (W = 1) from the SM-level shared-memory
-// pipe limit (W = 8, 16).  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -I effort_b200/csrc -o acc_rate acc_rate.cu
+// pipe limit (W = 8, 16).  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -I effort_b200/csrc -o acc_rate acc_rate.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -122,7 +122,7 @@ int main() {
     srand(7);
     for (auto& x : h) x = ((uint32_t)rand() << 16) ^ (uint32_t)rand();
     uint32_t* dw; long long* dc; float* ds;
-    cudaMalloc(&dw, h.size() * 4); cudaMalloc(&dc, 16 * 8 * 148); cudaMalloc(&ds, 64);
+    cudaMalloc(&dw, h.size() * 4); cudaMalloc(&dc, 16 * 8 * 132); cudaMalloc(&ds, 64);
     cudaMemcpy(dw, h.data(), h.size() * 4, cudaMemcpyHostToDevice);
     run<4, 0>(dw, dc, ds, "rmw N=4");
     run<2, 0>(dw, dc, ds, "rmw N=2");

@@ -78,14 +78,14 @@ void run(const uint32_t* dw, const unsigned char* src, size_t src_bytes, long lo
     const size_t smem = 8192 + 8 * 8192 + 8 * 4096 + 8 * 8192;
     cudaFuncSetAttribute(k<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const int iters = 400;
-    cudaMemset(dout, 0, 148 * 32 * 8);
+    cudaMemset(dout, 0, 132 * 32 * 8);
     k<MODE><<<grid, 512, smem>>>(dw, src, src_bytes, iters, on, unit_bytes, dout);
     cudaDeviceSynchronize();
-    cudaMemset(dout, 0, 148 * 32 * 8);
+    cudaMemset(dout, 0, 132 * 32 * 8);
     k<MODE><<<grid, 512, smem>>>(dw, src, src_bytes, iters, on, unit_bytes, dout);
     cudaError_t e = cudaDeviceSynchronize(); if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return; }
-    std::vector<long long> h(148 * 32);
+    std::vector<long long> h(132 * 32);
     cudaMemcpy(h.data(), dout, h.size() * 8, cudaMemcpyDeviceToHost);
     double cyc = 0, bytes = 0, pcyc = 0;
     for (int b = 0; b < grid; b++) {
@@ -106,10 +106,10 @@ int main() {
     for (auto& x : h) x = (((uint32_t)rand() << 16) ^ (uint32_t)rand()) & 0x3fff3fffu;
     uint32_t* dw; long long* dout; unsigned char* src;
     const size_t src_bytes = 32u << 20;
-    cudaMalloc(&dw, h.size() * 4); cudaMalloc(&dout, 148 * 32 * 8); cudaMalloc(&src, src_bytes);
+    cudaMalloc(&dw, h.size() * 4); cudaMalloc(&dout, 132 * 32 * 8); cudaMalloc(&src, src_bytes);
     cudaMemset(src, 0x3c, src_bytes);
     cudaMemcpy(dw, h.data(), h.size() * 4, cudaMemcpyHostToDevice);
-    for (int grid : {1, 148}) {
+    for (int grid : {1, 132}) {
         run<0>(dw, src, src_bytes, dout, 0, 4096, grid);
         for (int ub : {4096, 1536, 512}) {
             run<0>(dw, src, src_bytes, dout, 1, ub, grid);

@@ -2,7 +2,7 @@
 // 8-byte global loads into a register ring (B banks of 4 rows), an L2 prefetch runs PF units ahead, and every row goes
 // through the same shared-memory read-modify-write as bucket_mul_v4_kernel.  Question: does the SM reach the 8
 // wavefronts/row bound of the accumulate (instead of 12 with cp.async/TMA staging) and what DRAM rate results?
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I effort_b200/csrc -o stream_acc stream_acc.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I effort_b200/csrc -o stream_acc stream_acc.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -90,14 +90,14 @@ void run(const unsigned char* buf, size_t bytes, float* ds, int units_per_warp) 
     float best = 1e9f;
     for (int rep = 0; rep < 5; rep++) {
         cudaEventRecord(e0);
-        k<B, UR, PF, NW><<<148, NW * 32, smem>>>(buf, n_units_total, units_per_warp, ds);
+        k<B, UR, PF, NW><<<132, NW * 32, smem>>>(buf, n_units_total, units_per_warp, ds);
         cudaEventRecord(e1);
         cudaError_t e = cudaDeviceSynchronize();
         if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return; }
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         if (rep > 0 && ms < best) best = ms;
     }
-    const double total = 148.0 * NW * units_per_warp * UR * 256;
+    const double total = 132.0 * NW * units_per_warp * UR * 256;
     printf("banks %d (rows in flight %2d/warp)  unit %2d rows  prefetch %d units  warps %2d: %7.1f us  %6.0f GB/s  (%.1f MB)\n", B, B * 4, UR, PF, NW,
            best * 1e3, total / (best * 1e-3) / 1e9, total / 1e6);
 }
