@@ -80,9 +80,7 @@ struct V2Batch {
     int dynamic;             // 1: warps take units from a shared counter; 0: static round robin
     int ring_bytes;          // bucket_mul_v3_kernel: bytes of the producer's staging ring
     int prefetch;            // bucket_mul_v4_kernel: speculative L2 prefetch of the rows the hint selects
-    int lookahead;           // bucket_mul_v4_kernel: consumers test the next unit's barrier / fetch its descriptor early
     int trace_cycles;        // EFFORT_TRACE=2: only the cheap SM-cycle stamps (the global-timer stamps perturb the phases)
-    int window;              // bucket_mul_v4_kernel (bulk): most units a producer issues per window (1..8)
     int cta_begin[kMulBatchMax + 1];
     V2Problem p[kMulBatchMax];
 };

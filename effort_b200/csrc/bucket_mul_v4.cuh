@@ -6,18 +6,19 @@
 // and an STS), so everything that is not those six instructions has to leave the accumulating warps, and the serial
 // prologue has to shrink.
 //
-//  * 8 CONSUMER warps (0-7), each with a private 8 KB accumulator tile, do nothing but wait for a unit, read its rows
-//    and run the read-modify-writes (four rows = 16 independent updates per lane at a time); while a unit is accumulated
-//    the next slot's barrier is tested and its descriptor fetched;
-//  * 8 PRODUCER warps (8-15), one per consumer.  Units are whole inputs: thread j of the CTA turns input j's selection
-//    mask into record j of a direct-indexed list {first 16-byte piece, rows, multiplier} (slice-major layout: the ranks an
-//    input selects inside this CTA's column slice are contiguous).  Each pair owns a fixed 1/8 of the pass's selected rows
-//    in list order, so the same rows reach the same tile in the same order in every run.  BULK (default): a producer
-//    takes WINDOWS of its range (ramped sizes), hands out the pair's ring space by
-//    shuffles, tests all outstanding slots' barriers in parallel and lets every lane issue its own unit: descriptor +
-//    mbarrier.arrive.expect_tx + ONE cp.async.bulk of 256..4096 bytes.  !BULK: one unit per step, copied with 16-byte
-//    cp.async by all lanes, completion through cp.async.mbarrier.arrive.noinc.  The slot comes back through a second
-//    mbarrier.  Up to 8 x 16 KB are in flight per SM.
+//  * 8 CONSUMER warps (0-7), each with a private 8 KB accumulator tile, do nothing but wait for a chunk, read its rows
+//    and run the read-modify-writes (four rows = 16 independent updates per lane at a time);
+//  * 8 PRODUCER warps (8-15), one per consumer.  Thread j of the CTA turns input j's selection mask into record j of a
+//    direct-indexed list {first 16-byte piece, rows, multiplier, rows before} (slice-major layout: the ranks an input
+//    selects inside this CTA's column slice are contiguous).  Each pair owns a fixed 1/8 of the pass's selected rows in
+//    list order, so the same rows reach the same tile in the same order in every run.  The pair's rows fill a ring of
+//    four 4 KB chunks in order, one aligned block of 16 rows of the pass per chunk; a record that crosses a chunk
+//    boundary is cut there.  Each chunk has a full
+//    and an empty mbarrier: the handshake is paid per 16 rows, not per input (an input selects ~4 rows at effort 0.25).
+//    BULK (default): the producer stages every chunk with a free slot at once -- the whole first ring-full right after
+//    the list barrier -- one lane per chunk posting the chunk's bytes (arrive.expect_tx) and every lane issuing the
+//    cp.async.bulk of its record's piece.  !BULK: all lanes copy each piece with 16-byte cp.async, completion through
+//    cp.async.mbarrier.arrive.noinc.  Up to 8 x 16 KB are in flight per SM.
 //  * the exact-select cutoff runs on the EIGHT consumer warps (two per scheduler, 16 products per lane, a 256-thread
 //    named barrier per round) while the producers zero the tiles and run the overwrite protocol.
 //  * what bounds the kernel is the SM's shared-memory pipe (12 wavefronts per 128-weight row: tools/ubench), and at low
@@ -28,19 +29,14 @@
 namespace effort {
 
 constexpr int kV4Pairs = 8;                    // consumer / producer warp pairs
-constexpr int kV4Units = 16;                   // units in flight per pair (descriptor slots; a power of two)
-constexpr int kV4RingBytes = 16 * 1024;        // staging bytes per pair: a first-in-first-out byte ring
+constexpr int kV4Chunks = 4;                   // chunks per pair ring (a power of two)
+constexpr int kV4ChunkRows = 16;               // rows per chunk: 16 full-width 256-byte row slices
+constexpr int kV4ChunkBytes = kV4ChunkRows * 256;
+constexpr int kV4RingBytes = kV4Chunks * kV4ChunkBytes;  // staging bytes per pair (16 KB)
 constexpr int kV4SelWarps = 8;                                   // warps of the exact-select group (the consumers)
 constexpr int kSelVals = EFFORT_PROBES_MAX / (kV4SelWarps * 32);  // probe products per thread (16)
 constexpr int kSelKeys = kSelVals / 2, kSelChunks = kSelVals / 8; // packed bf16x2 registers; 8-value chunks
 static_assert(kSelVals * kV4SelWarps * 32 == EFFORT_PROBES_MAX && kSelChunks >= 1, "the group holds all 4096 products");
-
-struct __align__(16) V4Desc {
-    uint32_t off;      // byte offset of the unit's first row in the pair's ring
-    uint32_t n;        // rows (0 = stop marker)
-    float val;         // the input's multiplier
-    uint32_t charged;  // ring bytes the unit holds (incl. a wrap skip charged to it): what the producer takes back
-};
 
 struct V4Header {
     CutoffSmem cut;                      // bisect mode scratch
@@ -50,9 +46,8 @@ struct V4Header {
     int sel_rows;
     uint32_t warp_rows[kV2Threads / 32]; // rows selected by each warp's records (the split below)
     uint32_t start[kV4Pairs + 1];        // start[q]: the record holding pair q's first row (start[kV4Pairs] = records)
-    unsigned long long full_bar[kV4Pairs][kV4Units];
-    unsigned long long empty_bar[kV4Pairs][kV4Units];
-    V4Desc desc[kV4Pairs][kV4Units];
+    unsigned long long full_bar[kV4Pairs][kV4Chunks];
+    unsigned long long empty_bar[kV4Pairs][kV4Chunks];
 };
 
 struct V4Smem {
@@ -63,6 +58,29 @@ struct V4Smem {
                                      (size_t)kV2MaxInputs * 16 + 128 + (size_t)kV4Pairs * kV4RingBytes +
                                      1024 /* the consumers read (and ignore) up to three rows past a unit's end */;
 };
+
+// The ring of a pair: chunk s of the pair's sequence (counted across passes and rounds) uses slot s % kV4Chunks; its
+// full barrier completes phase s / kV4Chunks when its bytes have landed, its empty barrier the same phase when the
+// consumer has read them.
+__device__ __forceinline__ uint32_t v4_slot(uint32_t s) { return s & (kV4Chunks - 1); }
+__device__ __forceinline__ uint32_t v4_phase(uint32_t s) { return (s / kV4Chunks) & 1u; }
+
+// Lane `lane` takes record t + lane of the pass (when t + lane < r_end) and clips it to rows [c0, c1) of the pass.  Returns
+// the number of leading records that end inside [.., c1): the records a cursor at t is done with once rows up to c1 are
+// handled.  It is < 32 when the next record reaches past c1 (or the records run out): then rows [c0, c1) are complete.
+struct V4Piece {
+    uint32_t lo, hi;  // rows [lo, hi) of the pass (hi <= lo: nothing in [c0, c1))
+    uint4 rec;
+};
+__device__ __forceinline__ uint32_t v4_pieces(const uint4* ulist, uint32_t t, uint32_t r_end, uint32_t c0, uint32_t c1, int lane,
+                                              V4Piece& pc) {
+    const bool have = t + (uint32_t)lane < r_end;
+    pc.rec = have ? ulist[t + lane] : make_uint4(0u, 0u, 0u, 0u);
+    pc.lo = max(pc.rec.w, c0);
+    pc.hi = min(pc.rec.w + pc.rec.y, c1);
+    const unsigned fin = __ballot_sync(0xffffffffu, have && pc.rec.w + pc.rec.y <= c1);  // a prefix: record ends never decrease
+    return fin == 0xffffffffu ? 32u : (uint32_t)(__ffs((int)~fin) - 1);
+}
 
 __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
@@ -236,9 +254,9 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
         }
     }
     if (warp == NC) {  // first producer warp: the ring barriers
-        for (int s = lane; s < NC * kV4Units; s += 32) {
-            // LDGSTS: 32 cp.async arrivals + the descriptor's; bulk copy: the expect_tx arrival (bytes complete the phase)
-            mbar_init((uint32_t)__cvta_generic_to_shared(&hdr.full_bar[0][0] + s), BULK ? 1 : 33);
+        for (int s = lane; s < NC * kV4Chunks; s += 32) {
+            // LDGSTS: the 32 lanes' cp.async arrivals; bulk copy: the expect_tx arrival (bytes complete the phase)
+            mbar_init((uint32_t)__cvta_generic_to_shared(&hdr.full_bar[0][0] + s), BULK ? 1 : 32);
             mbar_init((uint32_t)__cvta_generic_to_shared(&hdr.empty_bar[0][0] + s), 1);
         }
         if (lane == 0) hdr.sel_rows = 0;
@@ -259,16 +277,13 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     auto src_of = [&](int j) { return (uint32_t)(((size_t)e_no * pb.in * P * C + (size_t)(rsp + j * RS) * P * slice_cols) >> 3); };
     const uint32_t my_src0 = src_of(tid);
 
-    // debugging aid (EFFORT_TRACE): issue / arrival / release times of the first 80 units of pair 0 of CTA 0
+    // debugging aid (EFFORT_TRACE): issue / arrival / release times of the first 80 chunks of pair 0 of CTA 0
     unsigned long long* utrace = (pb.unit_trace && blockIdx.x == 0 && pair == 0) ? pb.unit_trace : nullptr;
     if (utrace && tid == 0) utrace[640] = (unsigned long long)clock64();  // time base: the SM's cycle counter
-    // pair state.  Both sides count units (seq); unit s uses descriptor slot s % kV4Units, barrier phase (s / kV4Units) & 1.
-    // Producer only: ring head, free bytes, oldest unit not yet reclaimed.
-    uint32_t seq = 0, tail_seq = 0, head = 0, free_b = kV4RingBytes;
-    uint32_t slot_charged = 0u;  // bulk producers: lane s remembers the ring bytes the unit in descriptor slot s holds
+    // pair state: both sides count the pair's chunks (seq) across passes and rounds
+    uint32_t seq = 0;
     const uint32_t full0 = (uint32_t)__cvta_generic_to_shared(&hdr.full_bar[pair][0]);
     const uint32_t empty0 = (uint32_t)__cvta_generic_to_shared(&hdr.empty_bar[pair][0]);
-    const uint32_t desc0 = (uint32_t)__cvta_generic_to_shared(&hdr.desc[pair][0]);
     V2_TRACE(1);
     pdl_wait();
     if (cst) cst[1] = (unsigned long long)clock64();
@@ -528,211 +543,163 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
                 }
                 __syncthreads();
             }
-            // this pair's part of record `rec`: rows [row_lo, row_hi) of the pass
-            auto clip = [&](uint4 rec) {
-                const uint32_t lo = max(rec.w, row_lo), hi = min(rec.w + rec.y, row_hi);
-                rec.x += (lo - rec.w) * rs16;
-                rec.y = hi > lo ? hi - lo : 0u;
-                return rec;
-            };
+            // the pair's rows [row_lo, row_hi) of the pass reach its ring in chunks: chunk c holds the pair's rows of
+            // [(kb + c) * kV4ChunkRows, (kb + c + 1) * kV4ChunkRows), kb = row_lo / kV4ChunkRows, row r at (r % kV4ChunkRows) *
+            // seg_bytes of the chunk's slot.  A record that crosses a chunk boundary is cut there, as the pair boundary cuts
+            // records.  The boundaries are multiples of kV4ChunkRows in the pass's rows, not the pair's: at high effort most
+            // records have 16 rows and start on such a multiple, so they stay whole -- four 4-row groups, not a cut pair of
+            // partial ones.
             const uint32_t r_next = hdr.start[pair + 1];
             const uint32_t r_end = r_next < nu_pass ? r_next + 1u : nu_pass;  // (the record holding the next pair's first row)
+            const uint32_t kb = row_lo / (uint32_t)kV4ChunkRows;
+            const uint32_t n_chunks = row_hi > row_lo ? (row_hi - 1u) / (uint32_t)kV4ChunkRows + 1u - kb : 0u;
+            auto chunk_lo = [&](uint32_t c) { return max((kb + c) * (uint32_t)kV4ChunkRows, row_lo); };
+            auto chunk_hi = [&](uint32_t c) { return min((kb + c + 1u) * (uint32_t)kV4ChunkRows, row_hi); };
+            auto chunk_of = [&](uint32_t r) { return r / (uint32_t)kV4ChunkRows - kb; };
+            auto at = [&](uint32_t r) { return (r % (uint32_t)kV4ChunkRows) * (uint32_t)seg_bytes; };  // byte offset of row r in its slot
+            const uint32_t seq0 = seq;  // chunk c of this round is chunk seq0 + c of the pair
+            seq += n_chunks;
             if (cst && j0 == 0) cst[7] = (unsigned long long)clock64();
             V2_TRACE(8);
 
-            if (!consumer && BULK) {
-                // ---- 3a. producer of pair `pair`, bulk copies.  Every shared-memory operation of a producer (record,
-                // barrier test, descriptor) queues behind the consumers' read-modify-writes -- the shared-memory pipe is the
-                // kernel's bottleneck (tools/ubench/stage_cost.cu: ~350 cycles per dependent operation) -- so a producer works
-                // on a WINDOW of units of its range at once, one per lane (1..8 units, ramped up), the records in
-                // parallel, ring space handed out by shuffles, the barrier tests of all outstanding slots in parallel, and each
-                // lane issues its own unit's descriptor + expect_tx + bulk copy. ----
-                auto reclaim = [&](bool block) {  // take back the bytes of every unit the consumer has released (in order)
-                    const uint32_t out_n = seq - tail_seq;
-                    const uint32_t rel = ((uint32_t)lane - tail_seq) & (kV4Units - 1);  // slot `lane`: distance from the oldest
-                    const bool mine = lane < kV4Units && rel < out_n;
-                    bool done = false;
-                    if (mine) {
-                        const uint32_t par = ((tail_seq + rel) / kV4Units) & 1u;
-                        done = mbar_test(empty0 + (uint32_t)lane * 8u, par);
-                        if (block && rel == 0 && !done) {
-                            done = mbar_wait_parked(empty0 + (uint32_t)lane * 8u, par);
-                            if (!done && pb.err_flag) atomicExch(pb.err_flag, 3u);
-                            done = true;  // (after the ~1 s bound: give up waiting, the error flag says so)
-                        }
-                    }
-                    const unsigned dm = __ballot_sync(0xffffffffu, done) & 0xFFFFu;
-                    const unsigned rot = ((dm | (dm << 16)) >> (tail_seq & (kV4Units - 1))) & 0xFFFFu;  // bit r: unit tail+r released
-                    const uint32_t n = min((uint32_t)(__ffs((int)~rot) - 1), out_n);
-                    const uint32_t got = __reduce_add_sync(0xffffffffu, (mine && rel < n) ? slot_charged : 0u);
-                    free_b += got;
-                    tail_seq += n;
-                };
-                uint32_t t0 = hdr.start[pair], grabs = 0u;
+            if (!consumer) {
+                // ---- 3a. producer of pair `pair`.  Every shared-memory operation of a producer queues behind the consumers'
+                // read-modify-writes (the shared-memory pipe bounds the kernel), so it stages every chunk that has a free slot
+                // at once -- the first ring-full right after the list barrier, then what the consumer has released -- with one
+                // record per lane, 32 records per step.  BULK: one lane per chunk posts the chunk's bytes (expect_tx), every
+                // lane issues the cp.async.bulk of its record's piece(s).  !BULK: all lanes copy each piece with 16-byte
+                // cp.async, completion through cp.async.mbarrier.arrive.noinc. ----
+                uint32_t t = hdr.start[pair];  // record cursor: the records before t are staged
 #pragma unroll 1
-                for (; t0 < r_end; t0 += min(min((uint32_t)batch.window, grabs), r_end - t0)) {
-                    // windows ramped up: the very first units must not queue behind a burst
-                    grabs++;
-                    const uint32_t cnt = min(min((uint32_t)batch.window, grabs), r_end - t0);
-                    uint4 rec = make_uint4(0u, 0u, 0u, 0u);
-                    if ((uint32_t)lane < cnt) rec = clip(ulist[t0 + lane]);
-                    const uint32_t my_bytes = rec.y * (uint32_t)seg_bytes;
-                    uint32_t pos = 0u;
-                    if (seq != tail_seq) reclaim(false);
-#pragma unroll 1
-                    while (pos < cnt) {
-                        // ring space for the window's records pos.. in order (warp-uniform arithmetic on broadcast sizes); empty
-                        // records are consumed without a slot
-                        uint32_t h = head, f = free_b, n_ok = 0u, n_seen = 0u, my_off = 0u, my_chg = 0u, my_k = 0xffffffffu;
-                        const uint32_t slots_free = (uint32_t)kV4Units - (seq - tail_seq);
-                        for (uint32_t l = pos; l < cnt; l++) {
-                            const uint32_t bts = __shfl_sync(0xffffffffu, my_bytes, (int)l);
-                            if (bts == 0u) { n_seen++; continue; }
-                            const uint32_t skip = (h + bts > (uint32_t)kV4RingBytes) ? ((uint32_t)kV4RingBytes - h) : 0u;
-                            if (f < bts + skip || n_ok >= slots_free) break;
-                            const uint32_t off = skip ? 0u : h;
-                            if ((uint32_t)lane == l) { my_off = off; my_chg = bts + skip; my_k = n_ok; }
-                            if ((uint32_t)lane == ((seq + n_ok) & (kV4Units - 1))) slot_charged = bts + skip;  // lane s keeps slot s
-                            h = off + bts;
-                            if (h >= (uint32_t)kV4RingBytes) h = 0u;
-                            f -= bts + skip;
-                            n_ok++;
-                            n_seen++;
+                for (uint32_t c = 0; c < n_chunks;) {
+                    // chunks c, c + 1, .. whose slots are free (chunk s reuses the slot of chunk s - kV4Chunks)
+                    const uint32_t s = seq0 + c + (uint32_t)lane;
+                    const bool free_slot = lane < kV4Chunks && c + (uint32_t)lane < n_chunks &&
+                                           (s < (uint32_t)kV4Chunks || mbar_test(empty0 + v4_slot(s) * 8u, v4_phase(s) ^ 1u));
+                    uint32_t k = (uint32_t)(__ffs((int)~__ballot_sync(0xffffffffu, free_slot)) - 1);
+                    if (k == 0u) {  // all in use: wait for the oldest
+                        const uint32_t so = seq0 + c;
+                        if (!mbar_wait_parked(empty0 + v4_slot(so) * 8u, v4_phase(so) ^ 1u) && pb.err_flag && lane == 0)
+                            atomicExch(pb.err_flag, 3u);
+                        k = 1u;  // (after the ~1 s bound: give up waiting, the error flag says so)
+                    }
+                    if ((uint32_t)lane < k) {
+                        const uint32_t cc = c + (uint32_t)lane;
+                        if (BULK) mbar_expect_tx(full0 + v4_slot(seq0 + cc) * 8u, (int)((chunk_hi(cc) - chunk_lo(cc)) * (uint32_t)seg_bytes));
+                        if (utrace && seq0 + cc < 80u) {
+                            utrace[8 * (seq0 + cc)] = (unsigned long long)clock64();
+                            utrace[8 * (seq0 + cc) + 3] = (unsigned long long)(chunk_hi(cc) - chunk_lo(cc));
                         }
-                        if (n_seen == 0u) { reclaim(true); continue; }
-                        if (my_k != 0xffffffffu) {
-                            const uint32_t slot = (seq + my_k) & (kV4Units - 1);
-                            const uint32_t fb = full0 + slot * 8u;
-                            asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(desc0 + slot * 16u), "r"(my_off), "r"(rec.y), "r"(rec.z),
-                                         "r"(my_chg) : "memory");
-                            if (utrace && seq + my_k < 80u) { utrace[8 * (seq + my_k)] = (unsigned long long)clock64(); utrace[8 * (seq + my_k) + 3] = (unsigned long long)rec.y; }
-                            mbar_expect_tx(fb, (int)my_bytes);
-                            bulk_g2s(ring_saddr + my_off, bk16 + rec.x, (int)my_bytes, fb, pol);
-                        }
-                        seq += n_ok;
-                        head = h;
-                        free_b = f;
-                        pos += n_seen;
                     }
-                }
-                // stop marker for the consumer
-                while (seq - tail_seq >= (uint32_t)kV4Units) reclaim(true);
-                {
-                    const uint32_t slot = seq & (kV4Units - 1);
-                    if (lane == 0) {
-                        asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(desc0 + slot * 16u), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-                        mbar_arrive(full0 + slot * 8u);
-                    }
-                    if ((uint32_t)lane == slot) slot_charged = 0u;
-                    seq++;
-                }
-            } else if (!consumer) {
-                // ---- 3a'. producer of pair `pair`, 16-byte cp.async by all lanes, one unit at a time ----
-                auto reclaim = [&]() {  // wait for the consumer to release the oldest unit, take its bytes back
-                    const uint32_t ts = tail_seq & (kV4Units - 1);
-                    if (!mbar_wait_parked(empty0 + ts * 8u, (tail_seq / kV4Units) & 1u)) {
-                        if (pb.err_flag && lane == 0) atomicExch(pb.err_flag, 3u);
-                    }
-                    free_b += hdr.desc[pair][ts].charged;
-                    tail_seq++;
-                };
-                auto fill = [&](uint32_t src16, uint32_t len, uint32_t valbits) {  // len rows (0 = stop marker) as the next unit
-                    const uint32_t bytes = len * (uint32_t)seg_bytes;
-                    const uint32_t skip = (head + bytes > (uint32_t)kV4RingBytes) ? ((uint32_t)kV4RingBytes - head) : 0u;
-                    while (free_b < bytes + skip || seq - tail_seq >= (uint32_t)kV4Units) reclaim();
-                    const uint32_t off = skip ? 0u : head;
-                    const uint32_t slot = seq & (kV4Units - 1);
-                    const uint32_t sa = ring_saddr + off;
-                    const uint32_t fb = full0 + slot * 8u;
-                    const uint4* src = bk16 + src16;
-                    if (lane == 0)
-                        asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(desc0 + slot * 16u), "r"(off), "r"(len), "r"(valbits),
-                                     "r"(bytes + skip) : "memory");
-                    if (utrace && lane == 0 && seq < 80u) { utrace[8 * seq] = (unsigned long long)clock64(); utrace[8 * seq + 3] = (unsigned long long)len; }
-                    const uint32_t pieces = len * rs16;
-                    const uint32_t d0 = sa + (uint32_t)lane * 16u;
-                    const uint4* s0p = src + lane;
-                    for (uint32_t q = (uint32_t)lane; q < pieces; q += 32u) cp_async16(d0 + (q - (uint32_t)lane) * 16u, s0p + (q - (uint32_t)lane), pol);
-                    cp_async_arrive_noinc(fb);  // arrives when this lane's copies have landed
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(fb);  // releases the descriptor
-                    seq++;
-                    head = off + bytes;
-                    free_b -= bytes + skip;
-                    if (head >= (uint32_t)kV4RingBytes) head = 0u;
-                };
+                    const uint32_t b0 = chunk_lo(c), b1 = chunk_hi(c + k - 1u);
 #pragma unroll 1
-                for (uint32_t t = hdr.start[pair]; t < r_end; t++) {
-                    const uint4 rec = clip(ulist[t]);
-                    if (rec.y != 0u) fill(rec.x, rec.y, rec.z);  // (an input that selected nothing left an empty record)
-                }
-                fill(0u, 0u, 0u);  // stop marker for the consumer
-            } else {
-                // ---- 3b. consumer: wait for the next unit of the pair's ring, read its rows, run the read-modify-writes ----
-                unsigned long long rows_done = 0ull;
-                bool nx_ok = false;  // the next unit had already landed when the current one was started: its descriptor is in nx_*
-                uint32_t nx_off = 0u, nx_n = 0u, nx_val = 0u;
-#pragma unroll 1
-                for (;;) {
-                    const uint32_t slot = seq & (kV4Units - 1);
-                    uint32_t hoff, hn, hv, hs;
-                    if (utrace && lane == 0 && seq < 80u) utrace[8 * seq + 1] = (unsigned long long)clock64();
-                    if (nx_ok) {
-                        hoff = nx_off; hn = nx_n; hv = nx_val;
-                    } else {
-                        if (!mbar_wait(full0 + slot * 8u, (seq / kV4Units) & 1u)) {
-                            if (pb.err_flag && lane == 0) atomicExch(pb.err_flag, 2u);
-                            break;
+                    for (;;) {  // the record pieces of rows [b0, b1), cut at chunk boundaries (records have <= 16 rows: two pieces at most)
+                        V4Piece pc;
+                        const uint32_t done = v4_pieces(ulist, t, r_end, b0, b1, lane, pc);
+                        if (BULK) {
+                            for (uint32_t lo = pc.lo; lo < pc.hi;) {
+                                const uint32_t cc = chunk_of(lo), sl = v4_slot(seq0 + cc);
+                                const uint32_t hi = min(pc.hi, chunk_hi(cc));
+                                bulk_g2s(ring_saddr + sl * (uint32_t)kV4ChunkBytes + at(lo),
+                                         bk16 + pc.rec.x + (lo - pc.rec.w) * rs16, (int)((hi - lo) * (uint32_t)seg_bytes), full0 + sl * 8u, pol);
+                                lo = hi;
+                            }
+                        } else {
+                            unsigned todo = __ballot_sync(0xffffffffu, pc.lo < pc.hi);
+                            while (todo) {
+                                const int l = __ffs((int)todo) - 1;
+                                todo &= todo - 1u;
+                                uint32_t lo = __shfl_sync(0xffffffffu, pc.lo, l);
+                                const uint32_t phi = __shfl_sync(0xffffffffu, pc.hi, l);
+                                uint32_t src = __shfl_sync(0xffffffffu, pc.rec.x, l) + (lo - __shfl_sync(0xffffffffu, pc.rec.w, l)) * rs16;
+                                while (lo < phi) {
+                                    const uint32_t cc = chunk_of(lo);
+                                    const uint32_t hi = min(phi, chunk_hi(cc));
+                                    const uint32_t d0 = ring_saddr + v4_slot(seq0 + cc) * (uint32_t)kV4ChunkBytes + at(lo);
+                                    const uint32_t n16 = (hi - lo) * rs16;
+                                    for (uint32_t q = (uint32_t)lane; q < n16; q += 32u) cp_async16(d0 + q * 16u, bk16 + src + q, pol);
+                                    src += n16;
+                                    lo = hi;
+                                }
+                            }
                         }
-                        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(hoff), "=r"(hn), "=r"(hv), "=r"(hs) : "r"(desc0 + slot * 16u));
+                        t += done;
+                        if (done < 32u) break;
                     }
-                    if (utrace && lane == 0 && seq < 80u) utrace[8 * seq + 2] = (unsigned long long)clock64();
-                    seq++;
-                    nx_ok = false;
-                    if (batch.lookahead && hn != 0u) {  // both round trips of the NEXT unit's hand-over overlap this unit's rows
-                        const uint32_t nslot = seq & (kV4Units - 1);
-                        nx_ok = mbar_test(full0 + nslot * 8u, (seq / kV4Units) & 1u);
-                        if (nx_ok)
-                            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(nx_off), "=r"(nx_n), "=r"(nx_val), "=r"(hs) : "r"(desc0 + nslot * 16u));
-                    }
-                    const int n = (int)hn;
-                    if (utrace && lane == 0 && seq <= 80u && n >= 0) utrace[8 * (seq - 1) + 4] = (unsigned long long)clock64();
-                    const uint32_t eb = empty0 + slot * 8u;
-                    if (n == 0) {
-                        if (lane == 0) mbar_arrive(eb);
+                    if (!BULK)
+                        for (uint32_t i = 0; i < k; i++) cp_async_arrive_noinc(full0 + v4_slot(seq0 + c + i) * 8u);  // when this lane's copies have landed
+                    c += k;
+                }
+            } else {
+                // ---- 3b. consumer: wait for the pair's next chunk, walk its record pieces, run the read-modify-writes ----
+                unsigned long long rows_done = 0ull;
+                uint32_t t = hdr.start[pair];  // record cursor: the records before t are accumulated
+#pragma unroll 1
+                for (uint32_t c = 0; c < n_chunks; c++) {
+                    const uint32_t s = seq0 + c, sl = v4_slot(s);
+                    const uint32_t c0 = chunk_lo(c), c1 = chunk_hi(c);
+                    const bool tr = utrace && lane == 0 && s < 80u;
+                    if (tr) utrace[8 * s + 1] = (unsigned long long)clock64();
+                    // the chunk's first 32 records are read while its bytes may still be on their way
+                    V4Piece pc;
+                    uint32_t done = v4_pieces(ulist, t, r_end, c0, c1, lane, pc);
+                    if (!mbar_wait(full0 + sl * 8u, v4_phase(s))) {
+                        if (pb.err_flag && lane == 0) atomicExch(pb.err_flag, 2u);
                         break;
                     }
-                    rows_done += (unsigned long long)n;
-                    const float val = __uint_as_float(hv);
-                    const uint32_t sa = ring_saddr + hoff;
-                    if (full_width) {
-                        uint32_t a0 = sa + (uint32_t)(lane * LB);
-                        int r = 0;
-                        for (; r + 4 <= n; r += 4, a0 += 4 * kRow) {
-                            accumulate_unit_fp16<VEC, 4, kRow>(base_lane, val, a0);
-                            if (utrace && lane == 0 && seq <= 80u && r == 0) utrace[8 * (seq - 1) + 5] = (unsigned long long)clock64();
+                    if (tr) utrace[8 * s + 2] = (unsigned long long)clock64();
+                    if (tr) utrace[8 * s + 4] = (unsigned long long)clock64();
+                    const uint32_t cbase = ring_saddr + sl * (uint32_t)kV4ChunkBytes;
+                    bool first = true;
+#pragma unroll 1
+                    for (;;) {
+                        unsigned todo = __ballot_sync(0xffffffffu, pc.lo < pc.hi);
+                        while (todo) {  // the pieces in list order: each is one input's rows, as a unit was before
+                            const int l = __ffs((int)todo) - 1;
+                            todo &= todo - 1u;
+                            const uint32_t lo = __shfl_sync(0xffffffffu, pc.lo, l);
+                            const int n = (int)(__shfl_sync(0xffffffffu, pc.hi, l) - lo);
+                            const float val = __uint_as_float(__shfl_sync(0xffffffffu, pc.rec.z, l));
+                            const uint32_t sa = cbase + at(lo);
+                            if (full_width) {
+                                // 4/3/2/1-row groups inside one record: rows of one input never alias in a tile word
+                                uint32_t a0 = sa + (uint32_t)(lane * LB);
+                                int r = 0;
+                                for (; r + 4 <= n; r += 4, a0 += 4 * kRow) accumulate_unit_fp16<VEC, 4, kRow>(base_lane, val, a0);
+                                switch (n - r) {
+                                    case 1: accumulate_unit_fp16<VEC, 1, kRow>(base_lane, val, a0); break;
+                                    case 2: accumulate_unit_fp16<VEC, 2, kRow>(base_lane, val, a0); break;
+                                    case 3: accumulate_unit_fp16<VEC, 3, kRow>(base_lane, val, a0); break;
+                                    default: break;
+                                }
+                            } else {
+                                // narrow slice: rows are seg_bytes apart, R rows per step, lanes past the slice idle.  A row's
+                                // rowslot (which half-tile sums it) is its index within the pair's piece of the record, k0 + r,
+                                // whether or not a chunk boundary cut the piece
+                                const int rowslot = lane / lpr, lcol = lane % lpr;  // (computed here: a division the common path never pays)
+                                const bool col_ok = lcol * VEC < slice_cols;
+                                const int k0 = (int)(lo - max(__shfl_sync(0xffffffffu, pc.rec.w, l), row_lo));
+                                for (int st = k0 / R; st * R < k0 + n; st++) {
+                                    const int r = st * R + rowslot;
+                                    const bool ok = (rowslot < R) && (r >= k0) && (r < k0 + n) && col_ok;
+                                    uint32_t ww[2] = {0u, 0u};
+                                    if (ok) asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(ww[0]), "=r"(ww[1]) : "r"(sa + (uint32_t)((r - k0) * seg_bytes + lcol * LB)));
+                                    accumulate_words<SLOTS, VEC>(base_lane, ok ? val : 0.f, ww);
+                                }
+                            }
+                            if (tr && first) utrace[8 * s + 5] = (unsigned long long)clock64();
+                            first = false;
                         }
-                        switch (n - r) {
-                            case 1: accumulate_unit_fp16<VEC, 1, kRow>(base_lane, val, a0); break;
-                            case 2: accumulate_unit_fp16<VEC, 2, kRow>(base_lane, val, a0); break;
-                            case 3: accumulate_unit_fp16<VEC, 3, kRow>(base_lane, val, a0); break;
-                            default: break;
-                        }
-                    } else {  // narrow slice: rows are seg_bytes apart, R rows per step, lanes past the slice idle
-                        const int rowslot = lane / lpr, lcol = lane % lpr;  // (computed here: a division the common path never pays)
-                        const bool col_ok = lcol * VEC < slice_cols;
-                        for (int st = 0; st * R < n; st++) {
-                            const int r = st * R + rowslot;
-                            const bool ok = (rowslot < R) && (r < n) && col_ok;
-                            uint32_t ww[2] = {0u, 0u};
-                            if (ok) asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(ww[0]), "=r"(ww[1]) : "r"(sa + (uint32_t)(r * seg_bytes + lcol * LB)));
-                            accumulate_words<SLOTS, VEC>(base_lane, ok ? val : 0.f, ww);
-                        }
+                        t += done;
+                        if (done < 32u) break;
+                        done = v4_pieces(ulist, t, r_end, c0, c1, lane, pc);
                     }
-                    if (utrace && lane == 0 && seq <= 80u) utrace[8 * (seq - 1) + 6] = (unsigned long long)clock64();
-                    __syncwarp();  // every lane has read the unit's bytes
-                    if (lane == 0) mbar_arrive(eb);
-                    if (utrace && lane == 0 && seq <= 80u) utrace[8 * (seq - 1) + 7] = (unsigned long long)clock64();
+                    rows_done += (unsigned long long)(c1 - c0);
+                    if (tr) utrace[8 * s + 6] = (unsigned long long)clock64();
+                    __syncwarp();  // every lane has read the chunk's bytes
+                    if (lane == 0) mbar_arrive(empty0 + sl * 8u);
+                    if (tr) utrace[8 * s + 7] = (unsigned long long)clock64();
                 }
                 if (lane == 0 && rows_done) atomicAdd(&hdr.sel_rows, (int)rows_done);  // rows selected = rows accumulated
                 if (pb.unit_trace && blockIdx.x == 0 && lane == 0) {  // when every consumer of CTA 0 ran dry, and how much it did

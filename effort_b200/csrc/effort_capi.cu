@@ -92,8 +92,6 @@ struct effort_ctx {
                                           // 2 = one TMA producer warp + byte ring (slice-major FP16 weights; measured slower)
                                           // 0 = per-warp cp.async rings, units of <= 4 rows (any layout, Q4)
     int engine = 2;                       // 2 = bucket_mul_v2_kernel, 1 = round-1 fused kernel + integrate
-    int lookahead = 1;                    // bucket_mul_v4 consumers: test the next slot and fetch its descriptor while the current unit is accumulated
-    int window = 8;                       // bucket_mul_v4 bulk producers: most units per window
     int prefetch = 0;                     // bucket_mul_v4: speculative L2 prefetch of the rows the previous cutoff selects
                                           // (measured: no gain at effort 0.25, -13 % at 1.0: the gather is not DRAM-latency bound)
     int use_hint = 1;                     // bucket_mul_v4: the select starts from the matrix's previous cutoff
@@ -165,8 +163,6 @@ extern "C" int effort_ctx_create(int device, effort_ctx_t** ctx_out) {
     { const char* e = getenv("EFFORT_ENGINE"); if (e && atoi(e) == 1) c->engine = 1; }
     { const char* e = getenv("EFFORT_DYN"); if (e) c->dynamic = atoi(e) ? 1 : 0; }
     { const char* e = getenv("EFFORT_PREFETCH"); if (e) c->prefetch = atoi(e) ? 1 : 0; }
-    { const char* e = getenv("EFFORT_LOOKAHEAD"); if (e) c->lookahead = atoi(e) ? 1 : 0; }
-    { const char* e = getenv("EFFORT_WINDOW"); if (e && atoi(e) >= 1 && atoi(e) <= 8) c->window = atoi(e); }
     { const char* e = getenv("EFFORT_HINT"); if (e) c->use_hint = atoi(e) ? 1 : 0; }
     if (getenv("EFFORT_TRACE")) {
         CK(cudaMalloc(&c->trace, sizeof(unsigned long long) * (16 * c->n_sms + 648 + 48 + 16)));
@@ -187,8 +183,6 @@ extern "C" int effort_ctx_set_option(effort_ctx_t* c, const char* name, int valu
     if (!strcmp(name, "engine")) { if (value != 1 && value != 2) return EFFORT_EINVAL; c->engine = value; return EFFORT_OK; }
     if (!strcmp(name, "stage")) { if (value != 0 && value != 2 && value != 3 && value != 4) return EFFORT_EINVAL; c->stage_mode = value; return EFFORT_OK; }
     if (!strcmp(name, "hint")) { if (value != 0 && value != 1) return EFFORT_EINVAL; c->use_hint = value; return EFFORT_OK; }
-    if (!strcmp(name, "lookahead")) { if (value != 0 && value != 1) return EFFORT_EINVAL; c->lookahead = value; return EFFORT_OK; }
-    if (!strcmp(name, "window")) { if (value < 1 || value > 8) return EFFORT_EINVAL; c->window = value; return EFFORT_OK; }
     if (!strcmp(name, "prefetch")) { if (value != 0 && value != 1) return EFFORT_EINVAL; c->prefetch = value; return EFFORT_OK; }
     if (!strcmp(name, "dynamic")) { if (value != 0 && value != 1) return EFFORT_EINVAL; c->dynamic = value; return EFFORT_OK; }
     return EFFORT_EINVAL;
@@ -565,9 +559,7 @@ static int launch_v2_batch(effort_ctx* ctx, const V2Call* calls, int n, int slot
     using L = V2Smem<SLOTS, VEC>;
     batch.dynamic = ctx->dynamic;
     batch.prefetch = ctx->prefetch;
-    batch.window = ctx->window;
     { static const int tc = [] { const char* e = getenv("EFFORT_TRACE"); return e && atoi(e) == 2 ? 1 : 0; }(); batch.trace_cycles = tc; }
-    batch.lookahead = ctx->lookahead;
     const size_t smem = L::bytes(batch.list_cap, D);
     if (smem > kMaxSmem) return EFFORT_ESHAPE;
     // every kernel needs its own opt-in to > 48 KB of dynamic shared memory (per device): keyed by the function pointer

@@ -86,20 +86,18 @@ int effort_ctx_set_cutoff_mode(effort_ctx_t* ctx, int mode);
 /* Tuning / A-B knobs of the fused operator (tests and tools; every value computes the same operator):
  *   "engine"   2 (default) round-2 kernel: one launch per group, staged streaming, reductions into `out`;
  *              1 round-1 kernel + integrate launch (deterministic fp32 order)
- *   "stage"    4 (default) eight consumer warps accumulate, eight producer warps stage whole-input units (1..16 rows)
- *              with bulk async copies (cp.async.bulk, several units per producer step) into per-pair rings and hand them over
- *              through mbarriers (slice-major FP16 weights; other weights take stage 0); 3 the same pairs fed by 16-byte
- *              cp.async, one unit per producer step; 2 one TMA producer warp, a shared byte ring and 16 consumers (measured
+ *   "stage"    4 (default) eight consumer warps accumulate, eight producer warps stage each pair's rows into a ring of
+ *              four 16-row chunks with bulk async copies (cp.async.bulk, one per record piece) and hand the chunks over
+ *              through mbarriers (slice-major FP16 weights; other weights take stage 0); 3 the same pairs and chunks fed by
+ *              16-byte cp.async; 2 one TMA producer warp, a shared byte ring and 16 consumers (measured
  *              slower: the single producer's serial issue is the limit); 0 sixteen self-serving warps with private cp.async
  *              rings, units of at most 4 rows
- *   "window"   1..8 (default 8) stage 4: most units a producer takes per ticket grab
- *   "lookahead" 1 (default) / 0 stages 3-4: consumers test the next slot's barrier and fetch its descriptor early
  *   "dynamic"  per-warp rings (stage 0/1) only: 0 (default) static round robin of the units, 1 units from a shared counter
  *   "hint"     1 (default) stages 3-4: the exact select starts its search at the cutoff the same matrix produced on the
  *              previous call (3 rounds instead of 8 when it moved by less than 12 %; the result never depends on it)
  *   "prefetch" 0 (default) / 1 stages 3-4: while the cutoff is being computed, rows that the matrix's previous cutoff
  *              would select are prefetched into L2 (measured: no gain -- the gather is not DRAM-latency bound)
- * Returns EFFORT_EINVAL for an unknown name or value.  Environment defaults: EFFORT_ENGINE, EFFORT_STAGE (ldgsts|tma|pairs-ldgsts), EFFORT_WINDOW, EFFORT_LOOKAHEAD,
+ * Returns EFFORT_EINVAL for an unknown name or value.  Environment defaults: EFFORT_ENGINE, EFFORT_STAGE (ldgsts|tma|pairs-ldgsts),
  * EFFORT_DYN, EFFORT_PREFETCH, EFFORT_HINT. */
 int effort_ctx_set_option(effort_ctx_t* ctx, const char* name, int value);
 /* Non-zero once a kernel of this context gave up a bounded wait: its output is invalid.  1 = the overwrite protocol

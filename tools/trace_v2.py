@@ -1,5 +1,5 @@
 """Timeline of one isolated launch of the default fused kernel (bucket_mul_v4_kernel).  EFFORT_TRACE=1: per-CTA
-global-timer stamps of the phases + SM-cycle stamps of CTA 0 (prologue steps, every unit of pair 0, when each consumer
+global-timer stamps of the phases + SM-cycle stamps of CTA 0 (prologue steps, every chunk of pair 0, when each consumer
 ran dry).  EFFORT_TRACE=2: the cycle stamps only -- the global-timer reads perturb the serial prologue."""
 import argparse, ctypes as C, os, sys
 import numpy as np
@@ -55,12 +55,12 @@ for rep in range(3):
                "list barrier", "consumers done", "tiles reduced", "(v normalised", "constants", "loop top", "16 tests)"]
         print("   CTA 0 thread 0, SM cycles since kernel entry: " + "; ".join(f"{l} {int(c - cs[0])}" for l, c in zip(lab, cs) if c))
         fin = ub[648:696].astype(np.int64)
-        print("   consumers of CTA 0: ran dry at cycle / rows / units:",
+        print("   consumers of CTA 0: ran dry at cycle / rows / chunks:",
               "  ".join(f"{int(fin[w]) - base if fin[w] else -1}/{int(fin[16 + w])}/{int(fin[32 + w])}" for w in range(8)))
-        print("   units of pair 0, CTA 0 -- SM cycles since the CTA started: rows | producer issued | consumer: starts waiting, "
-              "barrier passed, descriptor read, first 4 rows done, all rows done, slot released")
+        print("   chunks of pair 0, CTA 0 -- SM cycles since the CTA started: rows | producer issued | consumer: starts waiting, "
+              "barrier passed, records read, first piece done, all rows done, slot released")
         for k in range(80):
             if u[k, 0] == 0:
                 break
             c = [int(u[k, j]) - base if u[k, j] else -1 for j in (0, 1, 2, 4, 5, 6, 7)]
-            print(f"     unit {k:2d}: {int(u[k,3]):2d} rows | {c[0]:6d} | {c[1]:6d} {c[2]:6d} {c[3]:6d} {c[4]:6d} {c[5]:6d} {c[6]:6d}")
+            print(f"     chunk {k:2d}: {int(u[k,3]):2d} rows | {c[0]:6d} | {c[1]:6d} {c[2]:6d} {c[3]:6d} {c[4]:6d} {c[5]:6d} {c[6]:6d}")

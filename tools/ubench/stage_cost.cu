@@ -111,7 +111,7 @@ int main() {
     cudaMemcpy(dw, h.data(), h.size() * 4, cudaMemcpyHostToDevice);
     for (int grid : {1, 132}) {
         run<0>(dw, src, src_bytes, dout, 0, 4096, grid);
-        for (int ub : {4096, 1536, 512}) {
+        for (int ub : {4096, 2048, 1536, 512}) {
             run<0>(dw, src, src_bytes, dout, 1, ub, grid);
             run<1>(dw, src, src_bytes, dout, 1, ub, grid);
         }
