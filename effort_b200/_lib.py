@@ -66,6 +66,8 @@ SIGNATURES = {
     "effort_model_set_graphs": (C.c_int, [vp, C.c_int]),
     "effort_model_set_fused_glue": (C.c_int, [vp, C.c_int]),
     "effort_model_set_chain": (C.c_int, [vp, C.c_int]),
+    "effort_model_set_sampler": (C.c_int, [vp, vp]),
+    "effort_sample": (C.c_int, [vp, vp, C.c_int, vp, C.c_uint32, vp, vp]),
     "effort_launch_count": (C.c_uint64, []),
     "effort_last_selected": (C.c_int, [vp, C.POINTER(C.c_uint32), vp]),
     "effort_loader_open": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(C.c_void_p)]),
@@ -91,6 +93,11 @@ class ModelConfig(C.Structure):
     _fields_ = [("dim", C.c_int), ("hidden_dim", C.c_int), ("n_layers", C.c_int), ("n_heads", C.c_int),
                 ("n_kv_heads", C.c_int), ("head_dim", C.c_int), ("vocab", C.c_int), ("max_seq", C.c_int),
                 ("rope_theta", C.c_float), ("norm_eps", C.c_float), ("tp_rank", C.c_int), ("tp_size", C.c_int)]
+
+
+class Sampler(C.Structure):
+    """effort_sampler_t"""
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int), ("top_p", C.c_float), ("seed", C.c_uint64)]
 
 
 class EffortError(RuntimeError):

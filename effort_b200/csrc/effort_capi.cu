@@ -20,6 +20,7 @@
 #include "convert.cuh"
 #include "cutoff.cuh"
 #include "q4.cuh"
+#include "sample.cuh"
 
 using namespace effort;
 
@@ -1216,6 +1217,12 @@ struct effort_model {
     uint64_t launches_per_token = 0;
     bool use_graphs = true;
     bool warmed = false;
+    // sampler (effort_model_set_sampler): the step's sample kernel reads `sampler_dev`, refreshed from the pinned
+    // `sampler_host` on the step's stream when it changed, so a graph replay sees new parameters without recapture
+    bool sampling = false, sampler_dirty = false;
+    effort_sampler_t* sampler_dev = nullptr;
+    effort_sampler_t* sampler_host = nullptr;   // pinned
+    cudaEvent_t sampler_copied = nullptr;       // the last copy out of sampler_host has run
     std::vector<void*> owned;
 };
 
@@ -1297,7 +1304,8 @@ extern "C" int effort_model_destroy(effort_model_t* m) {
     if (!m) return EFFORT_OK;
     for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
     for (void* p : m->owned) cudaFree(p);
-    cudaFreeHost(m->h_token); cudaFreeHost(m->h_next); cudaFreeHost(m->h_logits);
+    cudaFreeHost(m->h_token); cudaFreeHost(m->h_next); cudaFreeHost(m->h_logits); cudaFreeHost(m->sampler_host);
+    if (m->sampler_copied) cudaEventDestroy(m->sampler_copied);
     delete m;
     return EFFORT_OK;
 }
@@ -1376,6 +1384,57 @@ extern "C" int effort_model_set_chain(effort_model_t* m, int chain) {
     }
     m->chain = chain;
     return EFFORT_OK;
+}
+
+static bool sampler_valid(const effort_sampler_t* s) {
+    return s->temperature > 0.f && s->temperature <= 3.402823466e38f && s->top_k >= 0 && s->top_p > 0.f && s->top_p <= 1.f;
+}
+
+static int enqueue_sample(effort_ctx* ctx, const float* logits, int n, const effort_sampler_t& prm,
+                          const effort_sampler_t* prm_dev, const int* pos_dev, uint32_t position, int32_t* token,
+                          cudaStream_t s) {
+    static bool configured[64] = {false};
+    if (!configured[ctx->device & 63]) {
+        CK(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kSampleHistBytes + (int)(kSampleCache * sizeof(float))));
+        configured[ctx->device & 63] = true;
+    }
+    const size_t smem = kSampleHistBytes + (size_t)(n < kSampleCache ? n : kSampleCache) * sizeof(float);
+    CK(launch_pdl(sample_kernel, dim3(1), dim3(kSampleThreads), smem, s, logits, n, prm, prm_dev, pos_dev, position, token));
+    LAUNCHED();
+    return EFFORT_OK;
+}
+
+extern "C" int effort_sample(effort_ctx_t* ctx, const float* logits_dev, int n, const effort_sampler_t* s, uint32_t position,
+                             int32_t* token_dev, void* stream) {
+    if (!ctx || !logits_dev || !s || !token_dev || n <= 0 || !sampler_valid(s)) return EFFORT_EINVAL;
+    return enqueue_sample(ctx, logits_dev, n, *s, nullptr, nullptr, position, token_dev, (cudaStream_t)stream);
+}
+
+extern "C" int effort_model_set_sampler(effort_model_t* m, const effort_sampler_t* s) {
+    if (!m || (s && !sampler_valid(s))) return EFFORT_EINVAL;
+    if (m->sampling != (s != nullptr)) {  // the step's launch sequence changes
+        for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
+        m->graphs.clear();
+    }
+    m->sampling = s != nullptr;
+    if (!s) return EFFORT_OK;
+    if (!m->sampler_dev) {
+        int rc = model_alloc(m, m->sampler_dev, 1);
+        if (rc) return rc;
+        CK(cudaMallocHost(&m->sampler_host, sizeof(effort_sampler_t)));
+        CK(cudaEventCreateWithFlags(&m->sampler_copied, cudaEventDisableTiming));
+    }
+    CK(cudaEventSynchronize(m->sampler_copied));  // a copy still queued reads the pinned block
+    *m->sampler_host = *s;
+    m->sampler_dirty = true;
+    return EFFORT_OK;
+}
+
+// the sampler's kernel after the head / argmax that advanced pos: overwrites `next` with the draw
+static int model_enqueue_sample(effort_model* m, cudaStream_t s) {
+    if (!m->sampling) return EFFORT_OK;
+    return enqueue_sample(m->ctx, m->logits, m->cfg.vocab, *m->sampler_host, m->sampler_dev, m->pos, 0u, m->next, s);
 }
 
 extern "C" const float* effort_model_logits(const effort_model_t* m) { return m ? m->logits : nullptr; }
@@ -1481,7 +1540,8 @@ static int model_enqueue_token_v2(effort_model* m, double effort, cudaStream_t s
             if ((rc = launch_v2(ctx, &w2, 1, 0, s))) return rc;
         }
     }
-    return enqueue_head(m, m->h, m->norm, m->out_core, c.vocab, 0, m->logits, true, s);
+    if ((rc = enqueue_head(m, m->h, m->norm, m->out_core, c.vocab, 0, m->logits, true, s))) return rc;
+    return model_enqueue_sample(m, s);
 }
 
 // enqueue one token (no graph logic).  token lives in m->token (device).  With tp_size = G > 1 this rank holds
@@ -1541,7 +1601,7 @@ static int model_enqueue_token(effort_model* m, double effort, cudaStream_t s) {
         if ((rc = enqueue_basic_mul(m->out_normed, m->out_core, c.vocab, c.dim, m->logits, ctx->n_sms, s))) return rc;
         CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, (const float*)m->logits, c.vocab, m->next, m->pos));
         LAUNCHED();
-        return EFFORT_OK;
+        return model_enqueue_sample(m, s);
     }
     // tensor parallel with the one-shot NVLink collectives: the all-reduce of each row-parallel GEMV is fused with
     // the residual add and the following rmsNorm*w, the x2 all-gather with silu*mul (csrc/comm.cuh)
@@ -1624,7 +1684,7 @@ static int model_enqueue_token(effort_model* m, double effort, cudaStream_t s) {
     }
     CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, (const float*)m->logits, c.vocab, m->next, m->pos));
     LAUNCHED();
-    return EFFORT_OK;
+    return model_enqueue_sample(m, s);
 }
 
 extern "C" int effort_model_step(effort_model_t* m, const int32_t* token_dev, double effort, void* stream_) {
@@ -1635,6 +1695,11 @@ extern "C" int effort_model_step(effort_model_t* m, const int32_t* token_dev, do
     m->host_pos++;
     CK(cudaMemcpyAsync(m->token, token_dev ? (const void*)token_dev : (const void*)m->next, sizeof(int),
                        cudaMemcpyDeviceToDevice, s));
+    if (m->sampling && m->sampler_dirty) {
+        CK(cudaMemcpyAsync(m->sampler_dev, m->sampler_host, sizeof(effort_sampler_t), cudaMemcpyHostToDevice, s));
+        CK(cudaEventRecord(m->sampler_copied, s));
+        m->sampler_dirty = false;
+    }
     const int key = effort_q(effort, EFFORT_PROBES_COUNT);
     if (!m->use_graphs || s == nullptr) return model_enqueue_token(m, effort, s);  // legacy stream cannot capture
     auto it = m->graphs.find(key);

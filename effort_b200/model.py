@@ -350,6 +350,12 @@ class DecodeModel:
         """2 = fused round-2 chain (5 launches per layer, default), 1 = one kernel per reference op."""
         check(self._L.effort_model_set_chain(self._h, int(chain)), "effort_model_set_chain")
 
+    def set_sampler(self, temperature: Optional[float] = None, top_k: int = 0, top_p: float = 1.0, seed: int = 0):
+        """Draw each step's next token on the device (DESIGN.md section 4.6) instead of taking the argmax; None = greedy,
+        the default.  New parameters take effect at the next step without recapturing its CUDA graph."""
+        prm = None if temperature is None else _lib.Sampler(float(temperature), int(top_k), float(top_p), int(seed))
+        check(self._L.effort_model_set_sampler(self._h, None if prm is None else C.byref(prm)), "effort_model_set_sampler")
+
     def step(self, token: Optional[torch.Tensor] = None, effort: float = 0.25):
         """Enqueue one decode step (token: device int32[1]; None = previous prediction)."""
         check(self._L.effort_model_step(self._h, None if token is None else token.data_ptr(), float(effort),
@@ -365,6 +371,28 @@ class DecodeModel:
                                              C.byref(nxt), None if logits is None else logits.ctypes.data,
                                              ops._stream_ptr()), "effort_model_step_host")
         return int(nxt.value)
+
+    def generate(self, prompt: list[int], n_new: int, effort: float = 0.25) -> list[int]:
+        """Reset, feed `prompt`, then n_new - 1 further steps on the previous prediction; returns the n_new predicted
+        tokens (greedy, or drawn by the sampler).  Each step's token is copied into a device buffer on the current
+        stream; the host synchronises once, at the end."""
+        n_steps = len(prompt) + n_new - 1
+        if not prompt or n_new < 1:
+            raise ValueError("generate needs a non-empty prompt and n_new >= 1")
+        if n_steps > self.cfg.max_seq:
+            raise ValueError(f"prompt ({len(prompt)}) + n_new ({n_new}) - 1 steps exceed max_seq ({self.cfg.max_seq})")
+        toks = torch.tensor(prompt, dtype=torch.int32, device="cuda")
+        out = torch.empty(n_new, dtype=torch.int32, device="cuda")
+        nxt = _tensor_from_ptr(self._L.effort_model_next_token(self._h), 1, torch.int32)
+        self.reset()
+        for i in range(len(prompt)):
+            self.step(toks[i:i + 1], effort)
+        out[0:1].copy_(nxt)
+        for j in range(1, n_new):
+            self.step(None, effort)
+            out[j:j + 1].copy_(nxt)
+        torch.cuda.current_stream().synchronize()
+        return out.tolist()
 
     def logits(self) -> torch.Tensor:
         """Device logits of the last step as a torch view (copy)."""

@@ -20,7 +20,7 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import EffortError, MulArgs, check
+from ._lib import EffortError, MulArgs, Sampler, check
 
 KIND_FP16, KIND_Q4 = 0, 1
 NO_REPACK = 1
@@ -266,6 +266,19 @@ def lastSelected(ctx: Optional[Context] = None) -> int:
     n = C.c_uint32(0)
     check(ctx._L.effort_last_selected(ctx._h, C.byref(n), _stream_ptr()), "lastSelected")
     return int(n.value)
+
+
+def sample(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0, seed: int = 0, position: int = 0,
+           ctx: Optional[Context] = None) -> torch.Tensor:
+    """One draw from logits [V] f32 on the device (the rule of DESIGN.md section 4.6): temperature, top-k (0 = no limit),
+    top-p (1 = no limit), Philox counter `position` under `seed`.  Returns a device int32 tensor [1]; no host sync."""
+    ctx = ctx or default_context()
+    _need(logits, torch.float32, "logits")
+    out = torch.empty(1, dtype=torch.int32, device=logits.device)
+    prm = Sampler(float(temperature), int(top_k), float(top_p), int(seed))
+    check(ctx._L.effort_sample(ctx._h, logits.data_ptr(), logits.numel(), C.byref(prm), int(position), out.data_ptr(),
+                               _stream_ptr()), "sample")
+    return out
 
 
 def launchCount() -> int:

@@ -229,7 +229,8 @@ int effort_comm_all_gather(effort_ctx_t* ctx, const float* send_dev, float* recv
  * runNetwork(tokens:effort:)  runNetwork.swift:68-316, one token per call: per layer rmsNormFast*attnNorm,
  * expertMul x3 (wq,wk,wv), rope_mx + calcScores + softmax + sumScores, expertMul wo, residual, rmsNormFast*
  * ffnNorm, expertMul w1,w3, silu, expertMul w2, residual (:124-183); final rmsNorm*norm and the dense
- * lm_head basicMul (:206-209); greedy next token = top-1 (:235-257).  north_star keeps this orchestration in
+ * lm_head basicMul (:206-209); greedy next token = top-1 (:235-257), or a seeded draw once a sampler is set
+ * (effort_model_set_sampler).  north_star keeps this orchestration in
  * Swift; there is no Swift toolchain here, so the mirror lives behind the same C-ABI and a Swift build would
  * call the per-operator entry points above instead.  Dims follow main.swift:45-46,56,72-77.
  */
@@ -295,6 +296,38 @@ int effort_model_set_fused_glue(effort_model_t* m, int enable);
  * argmax); 1 = one kernel per reference op (runNetwork.swift:124-183 order).  Other configurations (tensor parallel,
  * Q4, round-1 engine) always use chain 1.  Environment default: EFFORT_CHAIN. */
 int effort_model_set_chain(effort_model_t* m, int chain);
+
+/*
+ * Sampling on the device (DESIGN.md section 4.6).  Greedy (the argmax above) stays the default.  With a sampler set,
+ * every step ends with one more kernel that overwrites the next token with a draw from the step's logits l[0..V):
+ *   1. order: a before b if l_a > l_b, or l_a == l_b (+0 == -0) and a < b; NaN is never drawn.  No finite maximum:
+ *      the first +inf if there is one (greedy's choice), else token 0.
+ *   2. top-k: S_k = the first K tokens of that order (ties cut by index, |S_k| = K); all V when K = 0 or K >= V.
+ *   3. m = max l; for i in S_k: w_i = expf((l_i - m) / T) in fp32 (IEEE subtraction and division),
+ *      q_i = floor(w_i * 2^32) as uint64 (the maximum weighs 2^32; q_i = 0, a relative probability below 2^-32, is
+ *      never drawn).
+ *   4. top-p: Q_k = sum of q over S_k; need = ceil((double)P * (double)Q_k); S = the shortest prefix of S_k, in the
+ *      order of 1, whose sum of q reaches need.
+ *   5. x = word 0 of Philox4x32-10 with counter (position, 0, 0, 0) and key (seed & 0xffffffff, seed >> 32);
+ *      Q = sum of q over S; target = (x * Q) >> 32; the token is the smallest index in S whose inclusive prefix sum of
+ *      q over S, in INDEX order, exceeds target.
+ * Everything after the expf is integer arithmetic, so the draw depends only on the input bits.  In the model the
+ * position is the position after the step: the n-th step after effort_model_reset draws with position n.
+ */
+typedef struct {
+    float temperature;  /* T > 0, finite */
+    int top_k;          /* K >= 0; 0 = no limit */
+    float top_p;        /* P in (0, 1]; 1 = no limit */
+    uint64_t seed;
+} effort_sampler_t;
+/* NULL = greedy (the default).  Parameters are copied; a change of parameters takes effect at the next step without
+ * recapturing the step's CUDA graph; switching between greedy and sampling drops the captured graphs.  EFFORT_EINVAL
+ * for a NaN, infinite or non-positive temperature, top_k < 0, or top_p outside (0, 1]. */
+int effort_model_set_sampler(effort_model_t* m, const effort_sampler_t* s);
+/* Test hook: one draw from logits_dev[0..n) with `position` as the Philox counter into token_dev (device int32).
+ * Enqueue-only; the same kernel the model runs.  EFFORT_EINVAL for n <= 0 and the parameter errors above. */
+int effort_sample(effort_ctx_t* ctx, const float* logits_dev, int n, const effort_sampler_t* s, uint32_t position,
+                  int32_t* token_dev, void* stream);
 
 /* ---- introspection used by bench / tests -------------------------------- */
 /* number of kernels this library has launched since load (process-wide) */
