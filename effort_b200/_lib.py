@@ -68,6 +68,7 @@ SIGNATURES = {
     "effort_model_set_chain": (C.c_int, [vp, C.c_int]),
     "effort_model_set_sampler": (C.c_int, [vp, vp]),
     "effort_sample": (C.c_int, [vp, vp, C.c_int, vp, C.c_uint32, vp, vp]),
+    "effort_model_buffer": (C.c_void_p, [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "effort_launch_count": (C.c_uint64, []),
     "effort_last_selected": (C.c_int, [vp, C.POINTER(C.c_uint32), vp]),
     "effort_loader_open": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -1214,6 +1214,10 @@ struct effort_model {
     int *h_token = nullptr, *h_next = nullptr;  // pinned
     float* h_logits = nullptr;                  // pinned
     std::map<int, cudaGraphExec_t> graphs;      // keyed by q = Int(4095*(1-effort))
+    // the token path of the last enqueued or replayed step (effort_model_buffer): 0 = none yet, 1 = one of the
+    // chain-1 paths (generic, fused glue, tensor parallel), 2 = the fused chain; and the path each graph captured
+    int path = 0;
+    std::map<int, int> graph_path;
     uint64_t launches_per_token = 0;
     bool use_graphs = true;
     bool warmed = false;
@@ -1439,6 +1443,41 @@ static int model_enqueue_sample(effort_model* m, cudaStream_t s) {
 
 extern "C" const float* effort_model_logits(const effort_model_t* m) { return m ? m->logits : nullptr; }
 extern "C" const int32_t* effort_model_next_token(const effort_model_t* m) { return m ? m->next : nullptr; }
+
+extern "C" const void* effort_model_buffer(const effort_model_t* m, int which, int layer, size_t* count) {
+    if (count) *count = 0;
+    if (!m || m->path == 0) return nullptr;
+    const auto& c = m->cfg;
+    const int G = c.tp_size;
+    const bool chain2 = m->path == 2;
+    const int b = (c.n_layers - 1) & 1;  // the fused chain's parity buffers of the last layer
+    const size_t q = (size_t)(c.n_heads / G) * c.head_dim, kv = (size_t)(c.n_kv_heads / G) * c.head_dim;
+    bool moe = false;
+    for (const auto& l : m->layers) moe = moe || l.gate != nullptr;
+    const void* p = nullptr;
+    size_t n = 0;
+    switch (which) {
+        case EFFORT_BUF_Q: p = chain2 ? m->xq2[b] : m->xq; n = q; break;
+        case EFFORT_BUF_K: p = chain2 ? m->xk2[b] : m->xk; n = kv; break;
+        case EFFORT_BUF_V: p = chain2 ? m->xv2[b] : m->xv; n = kv; break;
+        case EFFORT_BUF_ATTN: p = m->attn; n = q; break;
+        case EFFORT_BUF_KCACHE:
+        case EFFORT_BUF_VCACHE:
+            if (layer < 0 || layer >= c.n_layers) return nullptr;
+            p = which == EFFORT_BUF_KCACHE ? m->layers[layer].kc : m->layers[layer].vc;
+            n = (size_t)c.max_seq * kv;
+            break;
+        case EFFORT_BUF_HIDDEN: p = m->h; n = c.dim; break;
+        case EFFORT_BUF_NORMED: if (!chain2) { p = m->out_normed; n = c.dim; } break;
+        case EFFORT_BUF_GATE_IN: if (chain2 && moe) { p = m->h_keep; n = c.dim; } break;
+        case EFFORT_BUF_GATE_IDX: if (chain2 && moe) { p = m->gate_idx; n = 2; } break;
+        case EFFORT_BUF_GATE_VAL: if (chain2 && moe) { p = m->gate_val; n = 2; } break;
+        case EFFORT_BUF_POS: p = m->pos; n = 1; break;
+        default: return nullptr;
+    }
+    if (p && count) *count = n;
+    return p;
+}
 extern "C" size_t effort_model_bucket_bytes(const effort_model_t* m) {
     if (!m) return 0;
     size_t b = 0;
@@ -1555,6 +1594,7 @@ static int model_enqueue_token(effort_model* m, double effort, cudaStream_t s) {
     if (!m->norm) return EFFORT_ESTATE;
     int rc;
     const bool v2_chain = G == 1 && m->chain == 2 && ctx->engine == 2 && model_all_fp16_v2(m);
+    m->path = v2_chain ? 2 : 1;
     if (v2_chain) return model_enqueue_token_v2(m, effort, s);
     for (const auto& l : m->layers)
         if (l.gate) return EFFORT_ESTATE;  // expert routing lives in the fused chain only
@@ -1719,11 +1759,13 @@ extern "C" int effort_model_step(effort_model_t* m, const int32_t* token_dev, do
         CK(cudaGraphInstantiate(&ge, g, 0));
         CK(cudaGraphDestroy(g));
         m->graphs[key] = ge;
+        m->graph_path[key] = m->path;
         it = m->graphs.find(key);
         m->launches_per_token = g_launches.load() - l0;
         g_launches.store(l0);  // captured, not launched: the replay below counts them
     }
     CK(cudaGraphLaunch(it->second, s));
+    m->path = m->graph_path[key];
     g_launches.fetch_add(m->launches_per_token);  // kernels one replay launches
     return EFFORT_OK;
 }

@@ -410,6 +410,27 @@ class DecodeModel:
         ptr = self._L.effort_model_next_token(self._h)
         return int(_tensor_from_ptr(ptr, 1, torch.int32).cpu()[0])
 
+    BUFFERS = {"Q": 0, "K": 1, "V": 2, "ATTN": 3, "KCACHE": 4, "VCACHE": 5, "HIDDEN": 6, "NORMED": 7, "GATE_IN": 8,
+               "GATE_IDX": 9, "GATE_VAL": 10, "POS": 11}
+
+    def buffer_view(self, name: str, layer: int = -1) -> Optional[torch.Tensor]:
+        """A flat device view of one working buffer as the last step left it (effort_model_buffer; the names are its
+        EFFORT_BUF_* without the prefix), or None where the path that step took has no such buffer.  `layer` picks the
+        KCACHE / VCACHE layer (negative counts from the end).  The view is ordered on the current stream, and its
+        contents change with the next step: copy what must outlive it."""
+        if layer < 0:
+            layer += self.cfg.n_layers
+        n = C.c_size_t(0)
+        ptr = self._L.effort_model_buffer(self._h, self.BUFFERS[name], int(layer), C.byref(n))
+        if not ptr:
+            return None
+        return _tensor_from_ptr(ptr, n.value, torch.float32 if name not in ("GATE_IDX", "POS") else torch.int32)
+
+    def buffer(self, name: str, layer: int = -1) -> Optional[torch.Tensor]:
+        """A device copy of buffer_view(name, layer).  GATE_IDX comes back as int32 (the experts are < 64)."""
+        v = self.buffer_view(name, layer)
+        return None if v is None else v.clone()
+
     @property
     def bucket_bytes(self) -> int:
         return int(self._L.effort_model_bucket_bytes(self._h))

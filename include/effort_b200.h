@@ -329,6 +329,25 @@ int effort_model_set_sampler(effort_model_t* m, const effort_sampler_t* s);
 int effort_sample(effort_ctx_t* ctx, const float* logits_dev, int n, const effort_sampler_t* s, uint32_t position,
                   int32_t* token_dev, void* stream);
 
+/* Test hook: read-only device pointer to one of the model's working buffers as the last step left it, so that each
+ * kernel of the step can be checked on the inputs it actually consumed.  `count` (may be NULL) receives the element
+ * count.  NULL (count 0) when the buffer does not exist on the path the model last enqueued or replayed, or for a bad
+ * `which` / `layer`.  The caller synchronises the step's stream first; the pointer stays valid until the model is
+ * destroyed, and its contents until the next step. */
+#define EFFORT_BUF_Q 0        /* f32 [n_heads*128]: the last layer's q GEMV output before rope, as the attention read it */
+#define EFFORT_BUF_K 1        /* f32 [n_kv*128]: the same for k */
+#define EFFORT_BUF_V 2        /* f32 [n_kv*128]: the same for v */
+#define EFFORT_BUF_ATTN 3     /* f32 [n_heads][128]: the last layer's attention output */
+#define EFFORT_BUF_KCACHE 4   /* f32 [max_seq][n_kv][128]: `layer`'s roped key cache */
+#define EFFORT_BUF_VCACHE 5   /* f32 [max_seq][n_kv][128]: `layer`'s value cache */
+#define EFFORT_BUF_HIDDEN 6   /* f32 [dim]: the residual stream after the last layer (the final norm's input) */
+#define EFFORT_BUF_NORMED 7   /* f32 [dim]: rmsNorm(h) * norm, the lm_head's input; NULL on chain 2 (its head norms on load) */
+#define EFFORT_BUF_GATE_IN 8  /* f32 [dim]: the hidden state the last MoE layer's gate normalised; NULL without MoE */
+#define EFFORT_BUF_GATE_IDX 9 /* u32 [2]: that layer's two routed experts, the first one first */
+#define EFFORT_BUF_GATE_VAL 10/* f32 [2]: their softmax weights */
+#define EFFORT_BUF_POS 11     /* i32 [1]: the device position (tokens decoded since the last reset) */
+const void* effort_model_buffer(const effort_model_t* m, int which, int layer, size_t* count);
+
 /* ---- introspection used by bench / tests -------------------------------- */
 /* number of kernels this library has launched since load (process-wide) */
 uint64_t effort_launch_count(void);

@@ -26,6 +26,20 @@ def rope(x, pos, theta=1e6, hd=128):
     return out.reshape(-1)
 
 
+def attention(q, K, V):
+    """calcScores + softmax + sumScores for one token in fp32: q [n_heads, hd] (roped), K / V [T, n_kv, hd]; head h reads
+    KV head h // (n_heads / n_kv).  Returns [n_heads, hd]."""
+    n_heads, hd = q.shape
+    rep = n_heads // K.shape[1]
+    out = np.empty((n_heads, hd), np.float32)
+    for hh in range(n_heads):
+        sc = (K[:, hh // rep, :] @ q[hh]) / np.float32(np.sqrt(hd))   # dotSetScore2 aux.metal:445
+        p = np.exp(sc.astype(np.float32))                             # softmax without max (aux.metal:185-199)
+        p = p / p.sum()
+        out[hh] = p @ V[:, hh // rep, :]                              # sumScores32 aux.metal:379-393
+    return out
+
+
 class RefModel:
     """weights: list of layers, each dict name -> dict(buckets, stats, probes, in, out) + 'attn_norm','ffn_norm'."""
 
@@ -68,15 +82,7 @@ class RefModel:
             k = rope(xk, self.pos).reshape(self.n_kv, self.hd)
             self.kc[li].append(k)
             self.vc[li].append(xv.reshape(self.n_kv, self.hd).copy())
-            K = np.stack(self.kc[li])  # [T, n_kv, hd]
-            V = np.stack(self.vc[li])
-            out = np.empty((self.n_heads, self.hd), np.float32)
-            rep = self.n_heads // self.n_kv
-            for hh in range(self.n_heads):
-                sc = (K[:, hh // rep, :] @ q[hh]) / np.float32(np.sqrt(self.hd))   # dotSetScore2 aux.metal:445
-                p = np.exp(sc.astype(np.float32))                                  # softmax without max (aux.metal:185-199)
-                p = p / p.sum()
-                out[hh] = p @ V[:, hh // rep, :]                                   # sumScores32 aux.metal:379-393
+            out = attention(q, np.stack(self.kc[li]), np.stack(self.vc[li]))
             h = h + self._mul(out.reshape(-1), L["wo"], effort)
             fx = rmsnorm_mul(h, L["ffn_norm"])
             if "gate" in L:   # runNetwork.swift:185-200
