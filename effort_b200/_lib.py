@@ -17,6 +17,13 @@ class MulArgs(C.Structure):
                 ("out_dev", C.c_void_p), ("effort", C.c_double), ("v_cutoff_dev", C.c_void_p)]
 
 
+class FusedArgs(C.Structure):
+    """effort_fused_args_t"""
+    _fields_ = [("v_dev", C.c_void_p), ("x3_dev", C.c_void_p), ("norm_w_dev", C.c_void_p), ("norm_eps", C.c_float),
+                ("w", C.c_void_p), ("exp_no_dev", C.c_void_p), ("out_scale_dev", C.c_void_p), ("out_dev", C.c_void_p),
+                ("effort", C.c_double), ("accumulate", C.c_int)]
+
+
 # name -> (restype, argtypes); every symbol include/effort_b200.h declares
 SIGNATURES = {
     "effort_version": (C.c_int, []),
@@ -69,6 +76,8 @@ SIGNATURES = {
     "effort_model_set_sampler": (C.c_int, [vp, vp]),
     "effort_sample": (C.c_int, [vp, vp, C.c_int, vp, C.c_uint32, vp, vp]),
     "effort_model_buffer": (C.c_void_p, [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "effort_fused_mul_batch": (C.c_int, [vp, C.POINTER(FusedArgs), C.c_int, vp]),
+    "effort_last_problem": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_uint32), vp]),
     "effort_launch_count": (C.c_uint64, []),
     "effort_last_selected": (C.c_int, [vp, C.POINTER(C.c_uint32), vp]),
     "effort_loader_open": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(C.c_void_p)]),

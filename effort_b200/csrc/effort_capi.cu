@@ -98,6 +98,7 @@ struct effort_ctx {
     int use_hint = 1;                     // bucket_mul_v4: the select starts from the matrix's previous cutoff
     int dynamic = 0;                      // v2 per-warp rings: units from a shared counter (1) or static round robin (0, measured faster)
     int last_rs[8] = {0};                 // row splits of the last v2 launch per batch slot (effort_last_selected)
+    int last_slots = 0;                   // batch slots 0 .. last_slots-1 hold results of the last v2 launch group
     bool last_was_v2 = false;
     void* comm = nullptr;                  // ncclComm_t
     int comm_rank = 0, comm_world = 1;
@@ -603,6 +604,7 @@ static int launch_v2_batch(effort_ctx* ctx, const V2Call* calls, int n, int slot
     if (rc) return rc;
     LAUNCHED();
     ctx->last_was_v2 = true;
+    ctx->last_slots = slot0 + n;
     return EFFORT_OK;
 }
 
@@ -940,6 +942,40 @@ extern "C" int effort_last_selected(effort_ctx_t* ctx, uint32_t* n_selected, voi
         return EFFORT_OK;
     }
     CK(cudaMemcpy(n_selected, ctx->sizes + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return EFFORT_OK;
+}
+
+extern "C" int effort_fused_mul_batch(effort_ctx_t* ctx, const effort_fused_args_t* a, int n, void* stream) {
+    if (!ctx || !a || n < 1 || n > kMulBatchMax || ctx->engine != 2) return EFFORT_EINVAL;
+    V2Call calls[kMulBatchMax];
+    for (int k = 0; k < n; k++) {
+        const effort_fused_args_t& x = a[k];
+        int rc = check_mul_args(ctx, x.v_dev, x.w, x.out_dev, x.effort);
+        if (rc) return rc;
+        if (x.norm_w_dev && x.x3_dev) return EFFORT_EINVAL;
+        if (x.w->kind != EFFORT_KIND_FP16 || !x.w->buckets || !v2_supported(x.w)) return EFFORT_ESHAPE;
+        if (x.norm_w_dev && x.w->in != 8 * kV2Threads) return EFFORT_ESHAPE;
+        V2Call& c = calls[k];
+        c.v = x.v_dev; c.v2 = x.x3_dev; c.norm_w = (const __half*)x.norm_w_dev; c.norm_eps = x.norm_eps; c.w = x.w;
+        c.exp_no = x.exp_no_dev; c.out_scale = x.out_scale_dev; c.out = x.out_dev; c.effort = x.effort;
+        c.out_mode = x.accumulate ? kOutAccumulate : kOutOverwrite;
+    }
+    return launch_v2(ctx, calls, n, 0, (cudaStream_t)stream);
+}
+
+extern "C" int effort_last_problem(effort_ctx_t* ctx, int slot, float* cutoff, uint32_t* n_selected, void* stream) {
+    if (!ctx || slot < 0 || slot >= kMaxBatch) return EFFORT_EINVAL;
+    if (!ctx->last_was_v2 || slot >= ctx->last_slots) return EFFORT_ESTATE;
+    CK(cudaStreamSynchronize((cudaStream_t)stream));
+    if (cutoff) CK(cudaMemcpy(cutoff, ctx->cutoff + slot, sizeof(float), cudaMemcpyDeviceToHost));
+    if (n_selected) {
+        std::vector<uint32_t> c((size_t)ctx->last_rs[slot]);
+        CK(cudaMemcpy(c.data(), ctx->sel_counts + (size_t)slot * ctx->n_sms, sizeof(uint32_t) * c.size(),
+                      cudaMemcpyDeviceToHost));
+        uint32_t t = 0;
+        for (uint32_t x : c) t += x;
+        *n_selected = t;
+    }
     return EFFORT_OK;
 }
 

@@ -268,6 +268,36 @@ def lastSelected(ctx: Optional[Context] = None) -> int:
     return int(n.value)
 
 
+def fusedMulBatch(calls: Sequence[dict], ctx: Optional[Context] = None):
+    """One launch group of the fused decode chain (effort_fused_mul_batch).  Each call is a dict with
+    v, by, out, effort and optionally norm (fp16 [in]: input = rmsNorm(v) * norm), eps (1e-5), x3 (input = silu(v) * x3),
+    expNo (device uint32 scalar), scale (device f32 scalar: out (+)= scale * W(input)) and accumulate (False: overwrite)."""
+    ctx = ctx or default_context()
+    arr = (_lib.FusedArgs * len(calls))()
+    for k, c in enumerate(calls):
+        by, v, out = c["by"], c["v"], c["out"]
+        _check_vec(v, by.inSize, "v")
+        _check_vec(out, by.outSize, "out")
+        x3, norm, scale = c.get("x3"), c.get("norm"), c.get("scale")
+        if x3 is not None:
+            _check_vec(x3, by.inSize, "x3")
+        if norm is not None:
+            _need(norm, torch.float16, "norm")
+        if scale is not None:
+            _need(scale, torch.float32, "scale")
+        arr[k] = _lib.FusedArgs(v.data_ptr(), _ptr(x3), _ptr(norm), float(c.get("eps", 1e-5)), by._h, _ptr(c.get("expNo")),
+                                _ptr(scale), out.data_ptr(), float(c["effort"]), 1 if c.get("accumulate") else 0)
+    check(ctx._L.effort_fused_mul_batch(ctx._h, arr, len(calls), _stream_ptr()), "fusedMulBatch")
+
+
+def lastProblem(slot: int = 0, ctx: Optional[Context] = None) -> tuple[float, int]:
+    """(cutoff, selected rows) of batch slot `slot` of the last fused launch group on this context."""
+    ctx = ctx or default_context()
+    c, n = C.c_float(0), C.c_uint32(0)
+    check(ctx._L.effort_last_problem(ctx._h, int(slot), C.byref(c), C.byref(n), _stream_ptr()), "lastProblem")
+    return float(c.value), int(n.value)
+
+
 def sample(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0, seed: int = 0, position: int = 0,
            ctx: Optional[Context] = None) -> torch.Tensor:
     """One draw from logits [V] f32 on the device (the rule of DESIGN.md section 4.6): temperature, top-k (0 = no limit),

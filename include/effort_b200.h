@@ -348,6 +348,36 @@ int effort_sample(effort_ctx_t* ctx, const float* logits_dev, int n, const effor
 #define EFFORT_BUF_POS 11     /* i32 [1]: the device position (tokens decoded since the last reset) */
 const void* effort_model_buffer(const effort_model_t* m, int which, int layer, size_t* count);
 
+/* Test hook: one launch group of the fused chain (effort_model_set_chain 2), with the glue it applies on load.  Entry k
+ * computes, with x its input,
+ *     x = v                                 (plain: wo)
+ *     x = rmsNorm(v) * norm_w               (norm_w_dev != NULL: [q,k,v] and [w1,w3]; v is the residual stream h)
+ *     x = silu(v) * x3 = x3 * v / (1 + expf(-v))   (x3_dev != NULL: w2; v is x1)
+ *     out = s * W_e(x)  or  out += s * W_e(x)       (accumulate 0 / 1)
+ * where W_e is expert *exp_no_dev of w (expert 0 when NULL), s = *out_scale_dev (1 when NULL; the MoE gate value), and
+ * the rows are selected, and the cutoff taken, on the unscaled x.  rmsNorm(v) = v / sqrtf(sum(v^2) / 4096 + norm_eps).
+ * All n entries go into ONE launch with the chain's geometry and batch slots 0..n-1: the same kernel, mode, stage and
+ * row splits as the model's step on the same weights.  Enqueue-only.  EFFORT_EINVAL for n outside 1..4, a NULL pointer,
+ * effort outside [0, 1], norm and silu in one entry, or the round-1 engine; EFFORT_ESHAPE when the fused chain could not
+ * run the weights (not FP16 buckets the round-2 kernel takes, or norm with in != 4096). */
+typedef struct {
+    const float* v_dev;          /* input; with norm_w_dev: the residual h; with x3_dev: x1 */
+    const float* x3_dev;         /* non-NULL: input = silu(v) * x3 */
+    const void* norm_w_dev;      /* non-NULL: input = rmsNorm(v) * norm_w, fp16 [in], in == 4096 */
+    float norm_eps;
+    const effort_weights_t* w;
+    const uint32_t* exp_no_dev;  /* device expert index, NULL = 0 */
+    const float* out_scale_dev;  /* non-NULL: out (+)= scale * W(input); rows selected on the unscaled input */
+    float* out_dev;
+    double effort;
+    int accumulate;              /* 1: out += ..., 0: out = ... */
+} effort_fused_args_t;
+int effort_fused_mul_batch(effort_ctx_t* ctx, const effort_fused_args_t* a, int n, void* stream);
+/* The cutoff and the selected-row count of batch slot `slot` (0..7) of the last round-2 launch group on this ctx
+ * (effort_last_selected reads slot 0 only).  Synchronises `stream`.  EFFORT_ESTATE when the last launch was not one, or
+ * had no such slot. */
+int effort_last_problem(effort_ctx_t* ctx, int slot, float* cutoff, uint32_t* n_selected, void* stream);
+
 /* ---- introspection used by bench / tests -------------------------------- */
 /* number of kernels this library has launched since load (process-wide) */
 uint64_t effort_launch_count(void);
