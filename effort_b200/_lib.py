@@ -75,6 +75,10 @@ SIGNATURES = {
     "effort_model_set_chain": (C.c_int, [vp, C.c_int]),
     "effort_model_set_sampler": (C.c_int, [vp, vp]),
     "effort_sample": (C.c_int, [vp, vp, C.c_int, vp, C.c_uint32, vp, vp]),
+    "effort_score": (C.c_int, [vp, vp, C.c_int, vp, C.c_int, vp, vp]),
+    "effort_model_set_scoring": (C.c_int, [vp, C.c_int]),
+    "effort_model_set_score_targets": (C.c_int, [vp, vp, C.c_int, vp]),
+    "effort_model_scores": (C.c_void_p, [vp]),
     "effort_model_buffer": (C.c_void_p, [vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "effort_fused_mul_batch": (C.c_int, [vp, C.POINTER(FusedArgs), C.c_int, vp]),
     "effort_last_problem": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_uint32), vp]),

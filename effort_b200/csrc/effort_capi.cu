@@ -21,6 +21,7 @@
 #include "cutoff.cuh"
 #include "q4.cuh"
 #include "sample.cuh"
+#include "score.cuh"
 
 using namespace effort;
 
@@ -1263,6 +1264,10 @@ struct effort_model {
     effort_sampler_t* sampler_dev = nullptr;
     effort_sampler_t* sampler_host = nullptr;   // pinned
     cudaEvent_t sampler_copied = nullptr;       // the last copy out of sampler_host has run
+    // scoring (effort_model_set_scoring): the step's score kernel reads target row entry pos - 1 and writes that record
+    bool scoring = false;
+    int32_t* score_targets = nullptr;          // [max_seq], -1 = no target
+    effort_score_t* scores = nullptr;          // [max_seq]
     std::vector<void*> owned;
 };
 
@@ -1332,8 +1337,10 @@ static int model_create_buffers(effort_model* m, effort_ctx* ctx, const effort_m
     }
     if ((rc = model_alloc(m, m->head_cand, (size_t)ctx->n_sms * 8)) || (rc = model_alloc(m, m->head_ticket, 1)) ||
         (rc = model_alloc(m, m->gate_idx, 2)) || (rc = model_alloc(m, m->gate_val, 2)) ||
-        (rc = model_alloc(m, m->h_keep, (size_t)cfg->dim)))
+        (rc = model_alloc(m, m->h_keep, (size_t)cfg->dim)) || (rc = model_alloc(m, m->score_targets, cfg->max_seq)) ||
+        (rc = model_alloc(m, m->scores, cfg->max_seq)))
         return rc;
+    CK(cudaMemset(m->score_targets, 0xff, sizeof(int32_t) * cfg->max_seq));  // all -1: no target
     CK(cudaMallocHost(&m->h_token, sizeof(int)));
     CK(cudaMallocHost(&m->h_next, sizeof(int)));
     CK(cudaMallocHost(&m->h_logits, sizeof(float) * cfg->vocab));
@@ -1477,6 +1484,51 @@ static int model_enqueue_sample(effort_model* m, cudaStream_t s) {
     return enqueue_sample(m->ctx, m->logits, m->cfg.vocab, *m->sampler_host, m->sampler_dev, m->pos, 0u, m->next, s);
 }
 
+static int enqueue_score(const float* logits, int n, const int32_t* targets, int n_rec, const int* pos_dev, int grid,
+                         effort_score_t* out, cudaStream_t s) {
+    CK(launch_pdl(score_kernel, dim3(grid), dim3(kScoreThreads), 0, s, logits, n, targets, n_rec, pos_dev, out));
+    LAUNCHED();
+    return EFFORT_OK;
+}
+
+extern "C" int effort_score(effort_ctx_t* ctx, const float* logits_dev, int n, const int32_t* targets_dev, int n_targets,
+                            effort_score_t* out_dev, void* stream) {
+    if (!ctx || !logits_dev || !targets_dev || !out_dev || n <= 0 || n_targets <= 0) return EFFORT_EINVAL;
+    return enqueue_score(logits_dev, n, targets_dev, n_targets, nullptr, n_targets, out_dev, (cudaStream_t)stream);
+}
+
+extern "C" int effort_model_set_scoring(effort_model_t* m, int enable) {
+    if (!m) return EFFORT_EINVAL;
+    if (m->scoring != (enable != 0)) {  // the step's launch sequence changes
+        for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
+        m->graphs.clear();
+    }
+    m->scoring = enable != 0;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_model_set_score_targets(effort_model_t* m, const int32_t* targets_dev, int n, void* stream) {
+    if (!m || n < 0 || n > m->cfg.max_seq || (!targets_dev && n > 0)) return EFFORT_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n > 0) CK(cudaMemcpyAsync(m->score_targets, targets_dev, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, s));
+    if (n < m->cfg.max_seq) CK(cudaMemsetAsync(m->score_targets + n, 0xff, sizeof(int32_t) * (m->cfg.max_seq - n), s));
+    return EFFORT_OK;
+}
+
+extern "C" const effort_score_t* effort_model_scores(const effort_model_t* m) { return m ? m->scores : nullptr; }
+
+// the scorer's kernel last in the step (after the sampler's, if any): record pos - 1 from the step's logits
+static int model_enqueue_score(effort_model* m, cudaStream_t s) {
+    if (!m->scoring) return EFFORT_OK;
+    return enqueue_score(m->logits, m->cfg.vocab, m->score_targets, m->cfg.max_seq, m->pos, 1, m->scores, s);
+}
+
+// what every token path enqueues after the head / argmax that advanced pos
+static int model_enqueue_tail(effort_model* m, cudaStream_t s) {
+    int rc = model_enqueue_sample(m, s);
+    return rc ? rc : model_enqueue_score(m, s);
+}
+
 extern "C" const float* effort_model_logits(const effort_model_t* m) { return m ? m->logits : nullptr; }
 extern "C" const int32_t* effort_model_next_token(const effort_model_t* m) { return m ? m->next : nullptr; }
 
@@ -1616,7 +1668,7 @@ static int model_enqueue_token_v2(effort_model* m, double effort, cudaStream_t s
         }
     }
     if ((rc = enqueue_head(m, m->h, m->norm, m->out_core, c.vocab, 0, m->logits, true, s))) return rc;
-    return model_enqueue_sample(m, s);
+    return model_enqueue_tail(m, s);
 }
 
 // enqueue one token (no graph logic).  token lives in m->token (device).  With tp_size = G > 1 this rank holds
@@ -1677,7 +1729,7 @@ static int model_enqueue_token(effort_model* m, double effort, cudaStream_t s) {
         if ((rc = enqueue_basic_mul(m->out_normed, m->out_core, c.vocab, c.dim, m->logits, ctx->n_sms, s))) return rc;
         CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, (const float*)m->logits, c.vocab, m->next, m->pos));
         LAUNCHED();
-        return model_enqueue_sample(m, s);
+        return model_enqueue_tail(m, s);
     }
     // tensor parallel with the one-shot NVLink collectives: the all-reduce of each row-parallel GEMV is fused with
     // the residual add and the following rmsNorm*w, the x2 all-gather with silu*mul (csrc/comm.cuh)
@@ -1760,7 +1812,7 @@ static int model_enqueue_token(effort_model* m, double effort, cudaStream_t s) {
     }
     CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, (const float*)m->logits, c.vocab, m->next, m->pos));
     LAUNCHED();
-    return model_enqueue_sample(m, s);
+    return model_enqueue_tail(m, s);
 }
 
 extern "C" int effort_model_step(effort_model_t* m, const int32_t* token_dev, double effort, void* stream_) {

@@ -86,6 +86,7 @@ class DecodeModel:
         self.layers = []      # keeps ExpertWeights + norm tensors alive
         self.head = None
         self._next = C.c_int32(0)
+        self._scoring = False
 
     def __del__(self):
         try:
@@ -355,6 +356,69 @@ class DecodeModel:
         the default.  New parameters take effect at the next step without recapturing its CUDA graph."""
         prm = None if temperature is None else _lib.Sampler(float(temperature), int(top_k), float(top_p), int(seed))
         check(self._L.effort_model_set_sampler(self._h, None if prm is None else C.byref(prm)), "effort_model_set_sampler")
+
+    def set_scoring(self, enable: bool):
+        """Score every step on the device (DESIGN.md section 4.7): step p after reset writes record p of scores() from
+        target p of set_score_targets.  Off by default."""
+        check(self._L.effort_model_set_scoring(self._h, 1 if enable else 0), "effort_model_set_scoring")
+        self._scoring = bool(enable)
+
+    def set_score_targets(self, targets: Optional[torch.Tensor]):
+        """Targets (device int32 [n <= max_seq]; None = none) for scoring: entry p is the token that should follow the
+        input of step p.  The rest of the row becomes -1 (no target).  Ordered on the current stream; no recapture."""
+        n = 0 if targets is None else targets.numel()
+        if targets is not None:
+            ops._need(targets, torch.int32, "targets")
+        check(self._L.effort_model_set_score_targets(self._h, None if targets is None else targets.data_ptr(), n,
+                                                     ops._stream_ptr()), "effort_model_set_score_targets")
+
+    def scores(self) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """A device copy of the records [max_seq] as (argmax, rank, logprob) columns; record p is the one the last step
+        at position p wrote."""
+        ptr = self._L.effort_model_scores(self._h)
+        rec = _tensor_from_ptr(ptr, 3 * self.cfg.max_seq, torch.int32).clone().view(self.cfg.max_seq, 3)
+        return ops.score_columns(rec)
+
+    def score(self, tokens: list[int], effort: float = 0.25) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Teacher-force `tokens` from a reset and score each next one (runNetwork's returnPredictions, plus the
+        log-likelihood).  Returns host tensors: the greedy prediction after every token [n] (int32), the log-probability
+        [n - 1] (float32) and the rank [n - 1] (int32) of tokens[1:].  The host synchronises once, at the end; the scoring
+        state is restored."""
+        n = len(tokens)
+        if n < 1 or n > self.cfg.max_seq:
+            raise ValueError(f"score needs 1 <= len(tokens) <= max_seq ({self.cfg.max_seq}), got {n}")
+        was = self._scoring
+        toks = torch.tensor(tokens, dtype=torch.int32, device="cuda")
+        try:
+            self.set_scoring(True)
+            self.set_score_targets(toks[1:])
+            self.reset()
+            for i in range(n):
+                self.step(toks[i:i + 1], effort)
+            ptr = self._L.effort_model_scores(self._h)
+            rec = _tensor_from_ptr(ptr, 3 * n, torch.int32).view(n, 3).cpu()
+        finally:
+            self.set_scoring(was)
+        argmax, rank, logprob = ops.score_columns(rec)
+        return argmax.clone(), logprob[:n - 1].clone(), rank[:n - 1].clone()
+
+    def choose(self, prompt: list[int], candidates: list[int], effort: float = 0.25, top: int = 16) -> Optional[int]:
+        """runNetwork's limitLogits rule: feed `prompt` from a reset and rank the candidates against the last logits
+        (effort_score).  Returns the index of the lowest-ranked candidate (the first one on equal ranks) when its rank is
+        below `top`, else None (the reference's 99)."""
+        if not prompt or not candidates:
+            raise ValueError("choose needs a non-empty prompt and candidate list")
+        if len(prompt) > self.cfg.max_seq:
+            raise ValueError(f"prompt ({len(prompt)}) exceeds max_seq ({self.cfg.max_seq})")
+        toks = torch.tensor(prompt, dtype=torch.int32, device="cuda")
+        self.reset()
+        for i in range(len(prompt)):
+            self.step(toks[i:i + 1], effort)
+        logits = _tensor_from_ptr(self._L.effort_model_logits(self._h), self.cfg.vocab)
+        _, rank, _ = ops.score(logits, torch.tensor(candidates, dtype=torch.int32, device="cuda"), self.ctx)
+        r = rank.cpu()
+        best = int(torch.argmin(torch.where(r < 0, torch.iinfo(torch.int32).max, r)))   # no target (out of range) never wins
+        return best if 0 <= int(r[best]) < top else None
 
     def step(self, token: Optional[torch.Tensor] = None, effort: float = 0.25):
         """Enqueue one decode step (token: device int32[1]; None = previous prediction)."""

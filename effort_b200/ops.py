@@ -311,6 +311,24 @@ def sample(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: floa
     return out
 
 
+def score_columns(records: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """effort_score_t records held as int32 [n, 3] -> (argmax, rank, logprob) column views (logprob as float32)."""
+    return records[:, 0], records[:, 1], records[:, 2].view(torch.float32)
+
+
+def score(logits: torch.Tensor, targets: torch.Tensor, ctx: Optional[Context] = None):
+    """Score each target token against logits [V] f32 on the device (the rule of DESIGN.md section 4.7), one record per
+    target (device int32 [n]; outside [0, V) = no target).  Returns (argmax, ranks, logprobs), device tensors [n] (int32,
+    int32, float32); argmax is the greedy token in every record.  No host sync."""
+    ctx = ctx or default_context()
+    _need(logits, torch.float32, "logits")
+    _need(targets, torch.int32, "targets")
+    rec = torch.empty((targets.numel(), 3), dtype=torch.int32, device=logits.device)
+    check(ctx._L.effort_score(ctx._h, logits.data_ptr(), logits.numel(), targets.data_ptr(), targets.numel(), rec.data_ptr(),
+                              _stream_ptr()), "score")
+    return score_columns(rec)
+
+
 def launchCount() -> int:
     return int(_lib.load().effort_launch_count())
 

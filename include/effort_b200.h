@@ -230,7 +230,8 @@ int effort_comm_all_gather(effort_ctx_t* ctx, const float* send_dev, float* recv
  * expertMul x3 (wq,wk,wv), rope_mx + calcScores + softmax + sumScores, expertMul wo, residual, rmsNormFast*
  * ffnNorm, expertMul w1,w3, silu, expertMul w2, residual (:124-183); final rmsNorm*norm and the dense
  * lm_head basicMul (:206-209); greedy next token = top-1 (:235-257), or a seeded draw once a sampler is set
- * (effort_model_set_sampler).  north_star keeps this orchestration in
+ * (effort_model_set_sampler); per-position predictions and log-probabilities of given tokens (returnPredictions,
+ * :228-232) once scoring is on (effort_model_set_scoring).  north_star keeps this orchestration in
  * Swift; there is no Swift toolchain here, so the mirror lives behind the same C-ABI and a Swift build would
  * call the per-operator entry points above instead.  Dims follow main.swift:45-46,56,72-77.
  */
@@ -328,6 +329,40 @@ int effort_model_set_sampler(effort_model_t* m, const effort_sampler_t* s);
  * Enqueue-only; the same kernel the model runs.  EFFORT_EINVAL for n <= 0 and the parameter errors above. */
 int effort_sample(effort_ctx_t* ctx, const float* logits_dev, int n, const effort_sampler_t* s, uint32_t position,
                   int32_t* token_dev, void* stream);
+
+/*
+ * Scoring on the device (DESIGN.md section 4.7): one record per target token t against logits l[0..V) (fp32).
+ *   1. argmax: the greedy token, the lowest index of the maximum (NaN never wins; all NaN gives 0).
+ *   2. rank: with key = the sampler's order-preserving key (-0 == +0, NaN below -inf),
+ *      rank = #{i : key_i > key_t} + #{i < t : key_i == key_t}, exact.  Rank 0 means greedy would pick t.
+ *   3. logprob: m = max over the non-NaN logits.  When m is finite, S = sum over non-NaN i of expf(l_i - m), summed in
+ *      fp32 in a fixed order (per-thread strided sums over 1024 threads, a shuffle tree, then the 32 warps in index
+ *      order), and logprob = (l_t - m) - logf(S) with IEEE subtraction; a NaN or -inf target gives -inf.  When m is not
+ *      finite (all NaN, all -inf, or some +inf) logprob is NaN.
+ *   4. t outside [0, V) (-1 = no target): rank = -1, logprob = NaN; argmax is still written.
+ * A record depends only on the logits' bits and t, so scoring keeps the decode bit-reproducible.
+ */
+typedef struct {
+    int32_t argmax;
+    int32_t rank;
+    float logprob;
+} effort_score_t;
+/* Test hook and operator: score targets_dev[0..n_targets) (device int32) against logits_dev[0..n) into
+ * out_dev[0..n_targets), one CTA per target, with the kernel the model runs.  Enqueue-only.  EFFORT_EINVAL for a NULL
+ * pointer, n <= 0 or n_targets <= 0. */
+int effort_score(effort_ctx_t* ctx, const float* logits_dev, int n, const int32_t* targets_dev, int n_targets,
+                 effort_score_t* out_dev, void* stream);
+/* Off by default.  When on, every step ends with one more launch (after the sampler's, when one is set) that writes
+ * record p = (position after the step) - 1 of effort_model_scores() from target row entry p: step p after
+ * effort_model_reset scores the token the caller says follows its input.  Switching on or off drops the captured graphs. */
+int effort_model_set_scoring(effort_model_t* m, int enable);
+/* Enqueue a copy of targets_dev[0..n) (device int32) into the model's target row [max_seq] and set the rest to -1 (no
+ * target).  The row starts as all -1.  New targets need no graph recapture.  EFFORT_EINVAL for n < 0, n > max_seq, or
+ * a NULL targets_dev with n > 0. */
+int effort_model_set_score_targets(effort_model_t* m, const int32_t* targets_dev, int n, void* stream);
+/* Device records [max_seq]: record p is the one the last step at position p wrote; zero until then.  Reset does not
+ * clear them. */
+const effort_score_t* effort_model_scores(const effort_model_t* m);
 
 /* Test hook: read-only device pointer to one of the model's working buffers as the last step left it, so that each
  * kernel of the step can be checked on the inputs it actually consumed.  `count` (may be NULL) receives the element
