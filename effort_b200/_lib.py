@@ -66,6 +66,8 @@ SIGNATURES = {
     "effort_model_set_head": (C.c_int, [vp, vp, vp, vp]),
     "effort_model_reset": (C.c_int, [vp, vp]),
     "effort_model_step": (C.c_int, [vp, vp, C.c_double, vp]),
+    "effort_model_prefill": (C.c_int, [vp, vp, C.c_int, C.c_double, vp]),
+    "effort_bucket_mul_multi": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_double, vp, vp, vp]),
     "effort_model_step_host": (C.c_int, [vp, C.POINTER(C.c_int32), C.c_double, C.POINTER(C.c_int32), vp, vp]),
     "effort_model_logits": (C.c_void_p, [vp]),
     "effort_model_next_token": (C.c_void_p, [vp]),

@@ -22,6 +22,7 @@
 #include "q4.cuh"
 #include "sample.cuh"
 #include "score.cuh"
+#include "prefill.cuh"
 
 using namespace effort;
 
@@ -106,6 +107,12 @@ struct effort_ctx {
     unsigned char* p2p_local = nullptr;    // this rank's symmetric buffer
     void* p2p_peer[16] = {nullptr};        // mapped peers (own entry = p2p_local)
     bool p2p_ready = false;
+    // multi-token GEMV hook (effort_bucket_mul_multi); the model owns its own prefill scratch
+    float* pf_part = nullptr;
+    size_t pf_part_cap = 0;
+    uint32_t* pf_cnt = nullptr;
+    size_t pf_cnt_cap = 0;
+    float* pf_cut = nullptr;              // [kPrefillMax]
 };
 
 static constexpr int kMaxBatch = 8;
@@ -221,6 +228,7 @@ extern "C" int effort_ctx_destroy(effort_ctx_t* c) {
     cudaFree(c->cutoff); cudaFree(c->loops); cudaFree(c->sizes); cudaFree(c->dispatch);
     cudaFree(c->chunk_counts); cudaFree(c->partial); cudaFree(c->sel_counts);
     cudaFree(c->trace); cudaFree(c->v2_sync); cudaFree(c->v2_err); cudaFree(c->v4_part); cudaFree(c->v4_sync);
+    cudaFree(c->pf_part); cudaFree(c->pf_cnt); cudaFree(c->pf_cut);
     for (int p = 0; p < 16; p++)
         if (c->p2p_peer[p] && c->p2p_peer[p] != (void*)c->p2p_local) cudaIpcCloseMemHandle(c->p2p_peer[p]);
     cudaFree(c->p2p_local);
@@ -981,6 +989,78 @@ extern "C" int effort_last_problem(effort_ctx_t* ctx, int slot, float* cutoff, u
 }
 
 // ---------------------------------------------------------------------------------------------------
+// multi-token GEMV (csrc/prefill.cuh): out[t] = W(v[t]) for up to kPrefillMax inputs, each with its own cutoff
+// ---------------------------------------------------------------------------------------------------
+static bool prefill_supported(const effort_weights* w) {
+    return w && w->kind == EFFORT_KIND_FP16 && w->layout == kSliceMajor && w->bk_own && w->st16 && w->n_experts == 1 &&
+           w->n_probes == kPrefillProbes && w->in >= kPrefillProbes && w->P <= 16;
+}
+
+// the geometry is a function of the matrix and the device only, so a token's result does not depend on the chunk
+static PrefillProblem prefill_problem(const effort_ctx* ctx, const effort_weights* w, double effort, float* out, int accumulate) {
+    PrefillProblem p{};
+    p.bk = w->bk_own; p.st16 = w->st16; p.probes = w->probes;
+    p.in = w->in; p.C = w->C; p.P = w->P;
+    p.W = w->C < 128 ? w->C : 128;
+    p.CS = (w->C + p.W - 1) / p.W;
+    p.RS = ctx->n_sms / p.CS < 1 ? 1 : ctx->n_sms / p.CS;
+    p.k = w->n_probes - effort_q(effort, w->n_probes);
+    p.out = out; p.accumulate = accumulate;
+    return p;
+}
+
+// scratch of a group at T = kPrefillMax: partial-sum floats and count words
+static void prefill_scratch_need(const PrefillGroup& g, size_t* floats, size_t* counts) {
+    *floats = 0; *counts = 0;
+    for (int k = 0; k < g.n; k++) {
+        *floats += (size_t)g.p[k].RS * kPrefillMax * g.p[k].C * 16;
+        *counts += (size_t)g.p[k].RS * kPrefillMax;
+    }
+}
+
+// point each problem of the group at its share of the scratch and enqueue cutoff, GEMV and split reduction
+static int enqueue_prefill_group(effort_ctx* ctx, PrefillGroup& g, float* part, uint32_t* cnt, float* cut, cudaStream_t s) {
+    static bool configured[64] = {false};
+    if (!configured[ctx->device & 63]) {
+        CK(cudaFuncSetAttribute(prefill_mul_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPrefillMax * 16 * 4 * 32 * 4));
+        configured[ctx->device & 63] = true;
+    }
+    int ctas = 0;
+    for (int k = 0; k < g.n; k++) {
+        PrefillProblem& p = g.p[k];
+        p.part = part; p.cnt_part = cnt;
+        if (!p.cut) p.cut = cut + k * kPrefillMax;
+        part += (size_t)p.RS * g.T * p.C * 16;
+        cnt += (size_t)p.RS * g.T;
+        ctas += p.CS * p.RS;
+    }
+    CK(launch_pdl(prefill_cutoff_kernel, dim3(g.T, g.n), dim3(1024), 0, s, (const PrefillGroup)g));
+    LAUNCHED();
+    CK(launch_pdl(prefill_mul_kernel, dim3(ctas), dim3(32 * g.T), (size_t)g.T * 16 * 4 * 32 * 4, s, (const PrefillGroup)g));
+    LAUNCHED();
+    CK(launch_pdl(prefill_reduce_kernel, dim3(2 * ctx->n_sms), dim3(256), 0, s, (const PrefillGroup)g));
+    LAUNCHED();
+    return EFFORT_OK;
+}
+
+extern "C" int effort_bucket_mul_multi(effort_ctx_t* ctx, const float* v_dev, int n, const effort_weights_t* w, float* out_dev,
+                                       double effort, float* cutoff_dev, uint32_t* count_dev, void* stream) {
+    if (!ctx || !v_dev || !w || !out_dev || n < 1 || n > kPrefillMax || !(effort >= 0.0 && effort <= 1.0)) return EFFORT_EINVAL;
+    if (!prefill_supported(w)) return EFFORT_ESHAPE;
+    PrefillGroup g{};
+    g.n = 1; g.T = n; g.V = v_dev;
+    g.p[0] = prefill_problem(ctx, w, effort, out_dev, 0);
+    g.p[0].cut = cutoff_dev;
+    g.p[0].count = count_dev;
+    size_t nf, nc;
+    prefill_scratch_need(g, &nf, &nc);
+    int rc;
+    if ((rc = ensure(ctx->pf_part, ctx->pf_part_cap, nf)) || (rc = ensure(ctx->pf_cnt, ctx->pf_cnt_cap, nc))) return rc;
+    if (!ctx->pf_cut) CK(cudaMalloc(&ctx->pf_cut, sizeof(float) * kPrefillMax * kPrefillMaxProblems));
+    return enqueue_prefill_group(ctx, g, ctx->pf_part, ctx->pf_cnt, ctx->pf_cut, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // convert
 // ---------------------------------------------------------------------------------------------------
 extern "C" int effort_bucketize(const void* w_dev, int out_dim, int in_dim, void* buckets_dev, void* stats_dev,
@@ -1268,6 +1348,16 @@ struct effort_model {
     bool scoring = false;
     int32_t* score_targets = nullptr;          // [max_seq], -1 = no target
     effort_score_t* scores = nullptr;          // [max_seq]
+    // prefill (effort_model_prefill): chunk buffers [kPrefillMax][...] and the multi-token GEMV scratch, allocated once at
+    // their maximum size by the first prefill; graphs live in `graphs` under prefill_graph_key
+    bool pf_ready = false, pf_warmed = false, pf_scored = false;
+    float *pf_h = nullptr, *pf_xn = nullptr, *pf_q = nullptr, *pf_k = nullptr, *pf_v = nullptr, *pf_attn = nullptr,
+          *pf_x1 = nullptr, *pf_x3 = nullptr, *pf_x2 = nullptr, *pf_logits = nullptr, *pf_part = nullptr, *pf_cut = nullptr;
+    uint32_t* pf_cnt = nullptr;
+    int* pf_tok = nullptr;
+    int* pf_lens = nullptr;                    // {0, 1, .., kPrefillMax}: EFFORT_BUF_CHUNK_LEN points at entry T
+    int pf_len = 0;                            // length of the last chunk
+    std::map<int, uint64_t> pf_launches;       // kernels one replay of a prefill graph launches
     std::vector<void*> owned;
 };
 
@@ -1485,8 +1575,8 @@ static int model_enqueue_sample(effort_model* m, cudaStream_t s) {
 }
 
 static int enqueue_score(const float* logits, int n, const int32_t* targets, int n_rec, const int* pos_dev, int grid,
-                         effort_score_t* out, cudaStream_t s) {
-    CK(launch_pdl(score_kernel, dim3(grid), dim3(kScoreThreads), 0, s, logits, n, targets, n_rec, pos_dev, out));
+                         effort_score_t* out, cudaStream_t s, int ld = 0) {
+    CK(launch_pdl(score_kernel, dim3(grid), dim3(kScoreThreads), 0, s, logits, n, targets, n_rec, pos_dev, out, ld));
     LAUNCHED();
     return EFFORT_OK;
 }
@@ -1536,6 +1626,30 @@ extern "C" const void* effort_model_buffer(const effort_model_t* m, int which, i
     if (count) *count = 0;
     if (!m || m->path == 0) return nullptr;
     const auto& c = m->cfg;
+    if (m->path == 3 || (which >= EFFORT_BUF_CHUNK_Q && which <= EFFORT_BUF_CHUNK_LEN)) {  // the last prefill chunk
+        if (m->path != 3) return nullptr;
+        const size_t T = m->pf_len, kv = (size_t)c.n_kv_heads * c.head_dim;
+        const void* p = nullptr;
+        size_t n = 0;
+        switch (which) {
+            case EFFORT_BUF_KCACHE:
+            case EFFORT_BUF_VCACHE:
+                if (layer < 0 || layer >= c.n_layers) return nullptr;
+                p = which == EFFORT_BUF_KCACHE ? m->layers[layer].kc : m->layers[layer].vc;
+                n = (size_t)c.max_seq * kv;
+                break;
+            case EFFORT_BUF_POS: p = m->pos; n = 1; break;
+            case EFFORT_BUF_CHUNK_Q: p = m->pf_q; n = T * c.dim; break;
+            case EFFORT_BUF_CHUNK_K: p = m->pf_k; n = T * kv; break;
+            case EFFORT_BUF_CHUNK_V: p = m->pf_v; n = T * kv; break;
+            case EFFORT_BUF_CHUNK_ATTN: p = m->pf_attn; n = T * c.dim; break;
+            case EFFORT_BUF_CHUNK_LOGITS: if (m->pf_scored) { p = m->pf_logits; n = T * c.vocab; } break;
+            case EFFORT_BUF_CHUNK_LEN: p = m->pf_lens + T; n = 1; break;
+            default: return nullptr;
+        }
+        if (p && count) *count = n;
+        return p;
+    }
     const int G = c.tp_size;
     const bool chain2 = m->path == 2;
     const int b = (c.n_layers - 1) & 1;  // the fused chain's parity buffers of the last layer
@@ -1874,5 +1988,184 @@ extern "C" int effort_model_step_host(effort_model_t* m, const int32_t* token_ho
     CK(cudaStreamSynchronize(s));
     if (next_token_host) *next_token_host = *m->h_next;
     if (logits_host) memcpy(logits_host, m->h_logits, sizeof(float) * m->cfg.vocab);
+    return EFFORT_OK;
+}
+
+// ---- prefill: up to kPrefillMax tokens per pass (DESIGN.md section 4.8) ---------------------------------------------
+// Per layer: rmsNorm*w (T vectors) -> [q,k,v] multi-token GEMV -> chunk attention (appends T cache rows) -> wo accumulated
+// into the residual rows -> rmsNorm*w -> [w1,w3] -> silu*mul -> w2 accumulated into the residual rows.  Then the head on
+// the last row (or, with scoring, the dense lm_head for every row), the sampler and the scorer, as a step ends.
+static bool model_prefill_fused(const effort_model* m) {
+    if (m->cfg.tp_size != 1 || m->chain != 2 || m->ctx->engine != 2 || m->ctx->cutoff_mode != EFFORT_CUTOFF_SELECT ||
+        !m->norm || !model_all_fp16_v2(m))
+        return false;
+    for (const auto& l : m->layers) {
+        if (l.gate) return false;
+        for (const effort_weights* w : {l.wq, l.wk, l.wv, l.wo, l.w1, l.w2, l.w3})
+            if (!prefill_supported(w)) return false;
+    }
+    return true;
+}
+
+static int prefill_groups(effort_model* m, const effort_model::Layer& l, double effort, PrefillGroup g[4]) {
+    const effort_ctx* ctx = m->ctx;
+    for (int k = 0; k < 4; k++) g[k] = PrefillGroup{};
+    g[0].n = 3; g[0].V = m->pf_xn;
+    g[0].p[0] = prefill_problem(ctx, l.wq, effort, m->pf_q, 0);
+    g[0].p[1] = prefill_problem(ctx, l.wk, effort, m->pf_k, 0);
+    g[0].p[2] = prefill_problem(ctx, l.wv, effort, m->pf_v, 0);
+    g[1].n = 1; g[1].V = m->pf_attn;
+    g[1].p[0] = prefill_problem(ctx, l.wo, effort, m->pf_h, 1);
+    g[2].n = 2; g[2].V = m->pf_xn;
+    g[2].p[0] = prefill_problem(ctx, l.w1, effort, m->pf_x1, 0);
+    g[2].p[1] = prefill_problem(ctx, l.w3, effort, m->pf_x3, 0);
+    g[3].n = 1; g[3].V = m->pf_x2;
+    g[3].p[0] = prefill_problem(ctx, l.w2, effort, m->pf_h, 1);
+    return EFFORT_OK;
+}
+
+static int model_prefill_buffers(effort_model* m) {
+    if (m->pf_ready) return EFFORT_OK;
+    const auto& c = m->cfg;
+    const size_t T = kPrefillMax, kvd = (size_t)c.n_kv_heads * c.head_dim;
+    size_t nf = 0, nc = 0;
+    PrefillGroup g[4];
+    prefill_groups(m, m->layers[0], 1.0, g);  // every layer has the same shapes
+    for (auto& gr : g) {
+        size_t f, k;
+        prefill_scratch_need(gr, &f, &k);
+        nf = f > nf ? f : nf;
+        nc = k > nc ? k : nc;
+    }
+    int rc;
+    if ((rc = model_alloc(m, m->pf_h, T * c.dim)) || (rc = model_alloc(m, m->pf_xn, T * c.dim)) ||
+        (rc = model_alloc(m, m->pf_q, T * c.dim)) || (rc = model_alloc(m, m->pf_k, T * kvd)) ||
+        (rc = model_alloc(m, m->pf_v, T * kvd)) || (rc = model_alloc(m, m->pf_attn, T * c.dim)) ||
+        (rc = model_alloc(m, m->pf_x1, T * c.hidden_dim)) || (rc = model_alloc(m, m->pf_x3, T * c.hidden_dim)) ||
+        (rc = model_alloc(m, m->pf_x2, T * c.hidden_dim)) || (rc = model_alloc(m, m->pf_logits, T * c.vocab)) ||
+        (rc = model_alloc(m, m->pf_part, nf)) || (rc = model_alloc(m, m->pf_cnt, nc)) ||
+        (rc = model_alloc(m, m->pf_cut, (size_t)kPrefillMax * kPrefillMaxProblems)) || (rc = model_alloc(m, m->pf_tok, T)) ||
+        (rc = model_alloc(m, m->pf_lens, T + 1)))
+        return rc;
+    int lens[kPrefillMax + 1];
+    for (int i = 0; i <= kPrefillMax; i++) lens[i] = i;
+    CK(cudaMemcpy(m->pf_lens, lens, sizeof(lens), cudaMemcpyHostToDevice));
+    // kernel attributes before any capture
+    CK(cudaFuncSetAttribute(chunk_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (2 * kChunkAttnTile + kChunkAttnPairs) * 128 * (int)sizeof(float)));
+    CK(cudaFuncSetAttribute(prefill_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)(T * c.dim * sizeof(__half))));
+    m->pf_ready = true;
+    return EFFORT_OK;
+}
+
+// one chunk of T tokens already in pf_tok, at the device position (no graph logic)
+static int model_enqueue_chunk(effort_model* m, double effort, int T, cudaStream_t s) {
+    const auto& c = m->cfg;
+    effort_ctx* ctx = m->ctx;
+    int rc;
+    CK(launch_pdl(prefill_embed_kernel, dim3(T), dim3(256), 0, s, (const int*)m->pf_tok, m->emb, c.dim, c.vocab, m->pf_h));
+    LAUNCHED();
+    const int G = c.n_heads / c.n_kv_heads;
+    const dim3 attn_grid(c.n_kv_heads, (G * T + kChunkAttnPairs - 1) / kChunkAttnPairs);
+    const size_t attn_smem = (size_t)(2 * kChunkAttnTile + kChunkAttnPairs) * 128 * sizeof(float);
+    for (int li = 0; li < c.n_layers; li++) {
+        const auto& l = m->layers[li];
+        PrefillGroup g[4];
+        prefill_groups(m, l, effort, g);
+        for (auto& gr : g) gr.T = T;
+        CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)m->pf_h, l.attn_norm, c.dim, c.norm_eps, m->pf_xn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[0], m->pf_part, m->pf_cnt, m->pf_cut, s))) return rc;
+        CK(launch_pdl(chunk_attention_kernel, attn_grid, dim3(kChunkAttnThreads), attn_smem, s, (const float*)m->pf_q,
+                      (const float*)m->pf_k, (const float*)m->pf_v, T, l.kc, l.vc, (const int*)m->pos, c.n_heads, c.n_kv_heads,
+                      c.rope_theta, c.max_seq, m->pf_attn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[1], m->pf_part, m->pf_cnt, m->pf_cut, s))) return rc;
+        CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)m->pf_h, l.ffn_norm, c.dim, c.norm_eps, m->pf_xn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[2], m->pf_part, m->pf_cnt, m->pf_cut, s))) return rc;
+        const int nx = T * c.hidden_dim;
+        CK(launch_pdl(silu_mul_kernel, dim3((nx + 255) / 256), dim3(256), 0, s, (const float*)m->pf_x1, (const float*)m->pf_x3, nx,
+                      m->pf_x2));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[3], m->pf_part, m->pf_cnt, m->pf_cut, s))) return rc;
+    }
+    CK(launch_pdl(prefill_advance_kernel, dim3(1), dim3(1), 0, s, m->pos, T - 1));
+    LAUNCHED();
+    m->pf_scored = m->scoring;
+    if (m->scoring) {  // logits for every row: the dense lm_head on rmsNorm(h[t]) * norm, then greedy on the last row
+        CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)m->pf_h, m->norm, c.dim, c.norm_eps, m->pf_xn));
+        LAUNCHED();
+        int grid = (c.vocab + 7) / 8;
+        if (grid > ctx->n_sms * 2) grid = ctx->n_sms * 2;
+        CK(launch_pdl(prefill_head_kernel, dim3(grid), dim3(256), (size_t)T * c.dim * sizeof(__half), s, (const float*)m->pf_xn, T,
+                      m->out_core, c.vocab, c.dim, m->pf_logits, m->logits));
+        LAUNCHED();
+        CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, (const float*)m->logits, c.vocab, m->next, m->pos));
+        LAUNCHED();
+        if ((rc = model_enqueue_sample(m, s))) return rc;
+        // records p0 .. p0+T-1 from the chunk's rows (score_kernel: record pos - T + block)
+        return enqueue_score(m->pf_logits, c.vocab, m->score_targets, c.max_seq, m->pos, T, m->scores, s, c.vocab);
+    }
+    if ((rc = enqueue_head(m, m->pf_h + (size_t)(T - 1) * c.dim, m->norm, m->out_core, c.vocab, 0, m->logits, true, s))) return rc;
+    return model_enqueue_sample(m, s);
+}
+
+static int prefill_graph_key(double effort, int T) { return (T << 12) | effort_q(effort, EFFORT_PROBES_COUNT); }
+
+static int model_prefill_chunk(effort_model* m, double effort, int T, cudaStream_t s) {
+    if (!m->use_graphs || s == nullptr || !m->pf_warmed) {  // the first chunk runs eagerly, as the first step does
+        m->pf_warmed = m->pf_warmed || (m->use_graphs && s != nullptr);
+        m->path = 3; m->pf_len = T;
+        return model_enqueue_chunk(m, effort, T, s);
+    }
+    const int key = prefill_graph_key(effort, T);
+    auto it = m->graphs.find(key);
+    if (it == m->graphs.end()) {
+        cudaGraph_t g = nullptr;
+        const uint64_t l0 = g_launches.load();
+        CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+        int rc = model_enqueue_chunk(m, effort, T, s);
+        cudaError_t e = cudaStreamEndCapture(s, &g);
+        if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+        CK(e);
+        cudaGraphExec_t ge = nullptr;
+        CK(cudaGraphInstantiate(&ge, g, 0));
+        CK(cudaGraphDestroy(g));
+        m->graphs[key] = ge;
+        m->graph_path[key] = 3;
+        m->pf_launches[key] = g_launches.load() - l0;
+        g_launches.store(l0);
+        it = m->graphs.find(key);
+    }
+    CK(cudaGraphLaunch(it->second, s));
+    m->path = 3; m->pf_len = T; m->pf_scored = m->scoring;
+    g_launches.fetch_add(m->pf_launches[key]);
+    return EFFORT_OK;
+}
+
+extern "C" int effort_model_prefill(effort_model_t* m, const int32_t* tokens_dev, int n, double effort, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (!m || !tokens_dev || n < 1 || !(effort >= 0.0 && effort <= 1.0)) return EFFORT_EINVAL;
+    if (n > m->cfg.max_seq - m->host_pos) return EFFORT_ESTATE;  // the KV cache would overflow
+    int rc;
+    if (!model_prefill_fused(m)) {  // every other configuration steps: the same launches and bits as n steps
+        for (int i = 0; i < n; i++)
+            if ((rc = effort_model_step(m, tokens_dev + i, effort, stream_))) return rc;
+        return EFFORT_OK;
+    }
+    if ((rc = model_prefill_buffers(m))) return rc;
+    if (m->sampling && m->sampler_dirty) {
+        CK(cudaMemcpyAsync(m->sampler_dev, m->sampler_host, sizeof(effort_sampler_t), cudaMemcpyHostToDevice, s));
+        CK(cudaEventRecord(m->sampler_copied, s));
+        m->sampler_dirty = false;
+    }
+    for (int c0 = 0; c0 < n; c0 += kPrefillMax) {
+        const int T = n - c0 < kPrefillMax ? n - c0 : kPrefillMax;
+        CK(cudaMemcpyAsync(m->pf_tok, tokens_dev + c0, sizeof(int32_t) * T, cudaMemcpyDeviceToDevice, s));
+        m->host_pos += T;
+        if ((rc = model_prefill_chunk(m, effort, T, s))) return rc;
+    }
     return EFFORT_OK;
 }

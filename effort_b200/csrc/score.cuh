@@ -14,17 +14,20 @@ namespace effort {
 
 constexpr int kScoreThreads = 1024;
 
-// record r = blockIdx.x, or *pos_dev - 1 when pos_dev is non-null (the model's position after the head advanced it);
-// records outside [0, n_rec) are not written.  The target is targets[r]; outside [0, n) it means "no target".
+// record r = blockIdx.x, or *pos_dev - gridDim.x + blockIdx.x when pos_dev is non-null (the model's position after the
+// head advanced it: pos - 1 for a step, the chunk's positions for a prefill chunk); records outside [0, n_rec) are not
+// written.  The target is targets[r]; outside [0, n) it means "no target".  Block b reads the logits row
+// logits + b * ld (ld = 0: every record scores the same vector).
 __global__ void __launch_bounds__(kScoreThreads, 1)
 score_kernel(const float* __restrict__ logits, int n, const int32_t* __restrict__ targets, int n_rec,
-             const int* __restrict__ pos_dev, effort_score_t* __restrict__ out) {
+             const int* __restrict__ pos_dev, effort_score_t* __restrict__ out, int ld) {
     __shared__ float bv[32], ws[32];
     __shared__ int bi[32], wc[32];
     pdl_trigger();
     pdl_wait();
-    const int r = pos_dev ? *pos_dev - 1 : (int)blockIdx.x;
+    const int r = pos_dev ? *pos_dev - (int)gridDim.x + (int)blockIdx.x : (int)blockIdx.x;
     if (r < 0 || r >= n_rec) return;
+    logits += (size_t)blockIdx.x * ld;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int t = targets[r];
     const bool has_t = t >= 0 && t < n;

@@ -425,6 +425,17 @@ class DecodeModel:
         check(self._L.effort_model_step(self._h, None if token is None else token.data_ptr(), float(effort),
                                         ops._stream_ptr()), "effort_model_step")
 
+    def prefill(self, tokens, effort: float = 0.25):
+        """Enqueue `tokens` (a list of ints or a device int32 tensor) at the current position, as len(tokens) steps would:
+        up to 16 tokens per pass through the multi-token GEMV where the model runs the fused chain (effort_model_prefill),
+        plain steps otherwise.  No host synchronisation."""
+        if isinstance(tokens, torch.Tensor):
+            toks = tokens.to(device="cuda", dtype=torch.int32).contiguous()
+        else:
+            toks = torch.tensor(list(tokens), dtype=torch.int32, device="cuda")
+        check(self._L.effort_model_prefill(self._h, toks.data_ptr(), int(toks.numel()), float(effort), ops._stream_ptr()),
+              "effort_model_prefill")
+
     def step_host(self, token: Optional[int] = None, effort: float = 0.25, logits=None) -> int:
         """End-to-end step with host buffers: H2D token, decode, D2H next token (+ logits into a numpy array)."""
         tok = None
@@ -475,7 +486,8 @@ class DecodeModel:
         return int(_tensor_from_ptr(ptr, 1, torch.int32).cpu()[0])
 
     BUFFERS = {"Q": 0, "K": 1, "V": 2, "ATTN": 3, "KCACHE": 4, "VCACHE": 5, "HIDDEN": 6, "NORMED": 7, "GATE_IN": 8,
-               "GATE_IDX": 9, "GATE_VAL": 10, "POS": 11}
+               "GATE_IDX": 9, "GATE_VAL": 10, "POS": 11, "CHUNK_Q": 12, "CHUNK_K": 13, "CHUNK_V": 14, "CHUNK_ATTN": 15,
+               "CHUNK_LOGITS": 16, "CHUNK_LEN": 17}
 
     def buffer_view(self, name: str, layer: int = -1) -> Optional[torch.Tensor]:
         """A flat device view of one working buffer as the last step left it (effort_model_buffer; the names are its
@@ -488,7 +500,7 @@ class DecodeModel:
         ptr = self._L.effort_model_buffer(self._h, self.BUFFERS[name], int(layer), C.byref(n))
         if not ptr:
             return None
-        return _tensor_from_ptr(ptr, n.value, torch.float32 if name not in ("GATE_IDX", "POS") else torch.int32)
+        return _tensor_from_ptr(ptr, n.value, torch.float32 if name not in ("GATE_IDX", "POS", "CHUNK_LEN") else torch.int32)
 
     def buffer(self, name: str, layer: int = -1) -> Optional[torch.Tensor]:
         """A device copy of buffer_view(name, layer).  GATE_IDX comes back as int32 (the experts are < 64)."""

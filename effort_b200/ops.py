@@ -298,6 +298,22 @@ def lastProblem(slot: int = 0, ctx: Optional[Context] = None) -> tuple[float, in
     return float(c.value), int(n.value)
 
 
+def bucket_mul_multi(V: torch.Tensor, w: ExpertWeights, effort: float = 0.25, ctx: Optional[Context] = None):
+    """The prefill's multi-token GEMV (effort_bucket_mul_multi): V [T][in] float32 on the device, T <= 16.  Returns
+    (out [T][out], cutoffs [T] float32, counts [T] int32): each token's output, select-rule cutoff and selected-row count."""
+    ctx = ctx or default_context()
+    _need(V, torch.float32, "V")
+    if V.dim() != 2 or V.shape[1] != w.inSize:
+        raise ValueError(f"V must be [T][{w.inSize}], got {tuple(V.shape)}")
+    T = V.shape[0]
+    out = torch.empty(T, w.outSize, dtype=torch.float32, device=V.device)
+    cut = torch.empty(T, dtype=torch.float32, device=V.device)
+    cnt = torch.empty(T, dtype=torch.int32, device=V.device)
+    check(ctx._L.effort_bucket_mul_multi(ctx._h, V.data_ptr(), T, w._h, out.data_ptr(), float(effort), cut.data_ptr(),
+                                         cnt.data_ptr(), _stream_ptr()), "bucket_mul_multi")
+    return out, cut, cnt
+
+
 def sample(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0, seed: int = 0, position: int = 0,
            ctx: Optional[Context] = None) -> torch.Tensor:
     """One draw from logits [V] f32 on the device (the rule of DESIGN.md section 4.6): temperature, top-k (0 = no limit),

@@ -277,6 +277,16 @@ int effort_model_reset(effort_model_t* m, void* stream);
  * The first call for a given effort value runs eagerly and captures a CUDA graph; later calls replay it.
  */
 int effort_model_step(effort_model_t* m, const int32_t* token_dev, double effort, void* stream);
+/* Feed n known tokens (tokens_dev [n], device) at the current position, as n effort_model_step calls would: afterwards
+ * the position has advanced by n, the KV caches hold all n rows, effort_model_logits() holds the last position's logits
+ * and effort_model_next_token() greedy's choice (or the sampler's draw at position start + n); with scoring on, records
+ * start .. start+n-1 are written from the target row.  Enqueue-only.  Single-GPU FP16 models on the fused chain (chain 2,
+ * round-2 engine, select cutoff mode, slice-major weights, no MoE layer) run chunks of up to 16 tokens through the
+ * multi-token GEMV and a chunk attention (DESIGN.md section 4.8): the logits agree with stepping to the decode's bars,
+ * not bit for bit.  Every other configuration runs n effort_model_step calls.  CUDA graphs follow
+ * effort_model_set_graphs, one per (effort, chunk length).  EFFORT_EINVAL for n < 1, EFFORT_ESTATE when start + n >
+ * max_seq; nothing is enqueued in either case.  Out-of-range tokens are read as token 0, as a step reads them. */
+int effort_model_prefill(effort_model_t* m, const int32_t* tokens_dev, int n, double effort, void* stream);
 /* Same step driven with HOST buffers (the end-to-end call): token_host (NULL = previous prediction) is copied
  * H2D from pinned memory, the step runs, next token (and logits if logits_host != NULL) are copied D2H and the
  * stream is synchronised. */
@@ -381,6 +391,14 @@ const effort_score_t* effort_model_scores(const effort_model_t* m);
 #define EFFORT_BUF_GATE_IDX 9 /* u32 [2]: that layer's two routed experts, the first one first */
 #define EFFORT_BUF_GATE_VAL 10/* f32 [2]: their softmax weights */
 #define EFFORT_BUF_POS 11     /* i32 [1]: the device position (tokens decoded since the last reset) */
+/* The last effort_model_prefill chunk of T tokens (NULL unless the model's last call was a multi-token prefill; then
+ * EFFORT_BUF_KCACHE / _VCACHE / _POS are available too and the single-token ids above are NULL): */
+#define EFFORT_BUF_CHUNK_Q 12      /* f32 [T][n_heads*128]: the last layer's q GEMV outputs before rope */
+#define EFFORT_BUF_CHUNK_K 13      /* f32 [T][n_kv*128]: the same for k */
+#define EFFORT_BUF_CHUNK_V 14      /* f32 [T][n_kv*128]: the same for v */
+#define EFFORT_BUF_CHUNK_ATTN 15   /* f32 [T][n_heads*128]: the last layer's attention outputs */
+#define EFFORT_BUF_CHUNK_LOGITS 16 /* f32 [T][vocab]: every row's logits; only with scoring on */
+#define EFFORT_BUF_CHUNK_LEN 17    /* i32 [1]: T */
 const void* effort_model_buffer(const effort_model_t* m, int which, int layer, size_t* count);
 
 /* Test hook: one launch group of the fused chain (effort_model_set_chain 2), with the glue it applies on load.  Entry k
@@ -412,6 +430,16 @@ int effort_fused_mul_batch(effort_ctx_t* ctx, const effort_fused_args_t* a, int 
  * (effort_last_selected reads slot 0 only).  Synchronises `stream`.  EFFORT_ESTATE when the last launch was not one, or
  * had no such slot. */
 int effort_last_problem(effort_ctx_t* ctx, int slot, float* cutoff, uint32_t* n_selected, void* stream);
+
+/* Multi-token effort GEMV (the model's prefill kernel and geometry): out[t] = W(v[t]) for t < n <= 16 inputs
+ * (v_dev [n][in], out_dev [n][out], device).  Token t's cutoff is the EFFORT_CUTOFF_SELECT rule on its own probe
+ * products and its rows are those with cutoff[t] < (1e5 * stat) * |v[t][i]|, whatever the context's cutoff mode; out[t]
+ * is the fp32 sum of exactly those rows, in an order fixed by the matrix, so it repeats bit for bit and does not depend
+ * on the other inputs.  cutoff_dev [n] and count_dev [n] (may be NULL) receive each token's cutoff and selected-row
+ * count.  Enqueue-only.  EFFORT_EINVAL for n outside 1..16, a NULL pointer or effort outside [0, 1]; EFFORT_ESHAPE for
+ * weights other than single-expert FP16 buckets in the default slice-major layout with in >= 4096. */
+int effort_bucket_mul_multi(effort_ctx_t* ctx, const float* v_dev, int n, const effort_weights_t* w, float* out_dev,
+                            double effort, float* cutoff_dev, uint32_t* count_dev, void* stream);
 
 /* ---- introspection used by bench / tests -------------------------------- */
 /* number of kernels this library has launched since load (process-wide) */
