@@ -68,6 +68,18 @@ SIGNATURES = {
     "effort_model_step": (C.c_int, [vp, vp, C.c_double, vp]),
     "effort_model_prefill": (C.c_int, [vp, vp, C.c_int, C.c_double, vp]),
     "effort_bucket_mul_multi": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_double, vp, vp, vp]),
+    "effort_batch_create": (C.c_int, [vp, C.c_int, C.POINTER(C.c_void_p)]),
+    "effort_batch_destroy": (C.c_int, [vp]),
+    "effort_batch_reset": (C.c_int, [vp, C.c_int, vp]),
+    "effort_batch_fork": (C.c_int, [vp, C.c_int, vp]),
+    "effort_batch_step": (C.c_int, [vp, vp, C.c_double, vp]),
+    "effort_batch_set_sampler": (C.c_int, [vp, C.c_int, vp]),
+    "effort_batch_set_scoring": (C.c_int, [vp, C.c_int]),
+    "effort_batch_set_score_targets": (C.c_int, [vp, C.c_int, vp, C.c_int, vp]),
+    "effort_batch_logits": (C.c_void_p, [vp]),
+    "effort_batch_next_tokens": (C.c_void_p, [vp]),
+    "effort_batch_scores": (C.c_void_p, [vp]),
+    "effort_batch_buffer": (C.c_void_p, [vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "effort_model_step_host": (C.c_int, [vp, C.POINTER(C.c_int32), C.c_double, C.POINTER(C.c_int32), vp, vp]),
     "effort_model_logits": (C.c_void_p, [vp]),
     "effort_model_next_token": (C.c_void_p, [vp]),

@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libeffort_b200.so")
 SOURCES = ["effort_capi.cu", "safetensors_io.cpp"]
 HEADERS = ["common.cuh", "cutoff.cuh", "bucket_mul.cuh", "bucket_mul_v2.cuh", "bucket_mul_v3.cuh", "bucket_mul_v4.cuh",
-           "convert.cuh", "q4.cuh", "decode.cuh", "comm.cuh", "sample.cuh", "score.cuh", "prefill.cuh"]
+           "convert.cuh", "q4.cuh", "decode.cuh", "comm.cuh", "sample.cuh", "score.cuh", "prefill.cuh", "batch.cuh"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",

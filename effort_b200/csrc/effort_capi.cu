@@ -23,6 +23,7 @@
 #include "sample.cuh"
 #include "score.cuh"
 #include "prefill.cuh"
+#include "batch.cuh"
 
 using namespace effort;
 
@@ -2007,36 +2008,51 @@ static bool model_prefill_fused(const effort_model* m) {
     return true;
 }
 
-static int prefill_groups(effort_model* m, const effort_model::Layer& l, double effort, PrefillGroup g[4]) {
-    const effort_ctx* ctx = m->ctx;
+// the row buffers [T][...] one layer of multi-token groups reads and writes (a model's prefill chunk, or a batch step)
+struct RowBuffers {
+    float *h, *xn, *q, *k, *v, *attn, *x1, *x3, *x2;
+};
+
+static int row_groups(const effort_ctx* ctx, const effort_model::Layer& l, double effort, const RowBuffers& r, PrefillGroup g[4]) {
     for (int k = 0; k < 4; k++) g[k] = PrefillGroup{};
-    g[0].n = 3; g[0].V = m->pf_xn;
-    g[0].p[0] = prefill_problem(ctx, l.wq, effort, m->pf_q, 0);
-    g[0].p[1] = prefill_problem(ctx, l.wk, effort, m->pf_k, 0);
-    g[0].p[2] = prefill_problem(ctx, l.wv, effort, m->pf_v, 0);
-    g[1].n = 1; g[1].V = m->pf_attn;
-    g[1].p[0] = prefill_problem(ctx, l.wo, effort, m->pf_h, 1);
-    g[2].n = 2; g[2].V = m->pf_xn;
-    g[2].p[0] = prefill_problem(ctx, l.w1, effort, m->pf_x1, 0);
-    g[2].p[1] = prefill_problem(ctx, l.w3, effort, m->pf_x3, 0);
-    g[3].n = 1; g[3].V = m->pf_x2;
-    g[3].p[0] = prefill_problem(ctx, l.w2, effort, m->pf_h, 1);
+    g[0].n = 3; g[0].V = r.xn;
+    g[0].p[0] = prefill_problem(ctx, l.wq, effort, r.q, 0);
+    g[0].p[1] = prefill_problem(ctx, l.wk, effort, r.k, 0);
+    g[0].p[2] = prefill_problem(ctx, l.wv, effort, r.v, 0);
+    g[1].n = 1; g[1].V = r.attn;
+    g[1].p[0] = prefill_problem(ctx, l.wo, effort, r.h, 1);
+    g[2].n = 2; g[2].V = r.xn;
+    g[2].p[0] = prefill_problem(ctx, l.w1, effort, r.x1, 0);
+    g[2].p[1] = prefill_problem(ctx, l.w3, effort, r.x3, 0);
+    g[3].n = 1; g[3].V = r.x2;
+    g[3].p[0] = prefill_problem(ctx, l.w2, effort, r.h, 1);
     return EFFORT_OK;
+}
+
+// partial-sum floats and count words the largest group of a layer needs at T = kPrefillMax (every layer has the same shapes)
+static void row_scratch_need(const effort_model* m, size_t* nf, size_t* nc) {
+    *nf = 0; *nc = 0;
+    PrefillGroup g[4];
+    row_groups(m->ctx, m->layers[0], 1.0, RowBuffers{}, g);
+    for (auto& gr : g) {
+        size_t f, k;
+        prefill_scratch_need(gr, &f, &k);
+        *nf = f > *nf ? f : *nf;
+        *nc = k > *nc ? k : *nc;
+    }
+}
+
+static int prefill_groups(effort_model* m, const effort_model::Layer& l, double effort, PrefillGroup g[4]) {
+    return row_groups(m->ctx, l, effort,
+                      RowBuffers{m->pf_h, m->pf_xn, m->pf_q, m->pf_k, m->pf_v, m->pf_attn, m->pf_x1, m->pf_x3, m->pf_x2}, g);
 }
 
 static int model_prefill_buffers(effort_model* m) {
     if (m->pf_ready) return EFFORT_OK;
     const auto& c = m->cfg;
     const size_t T = kPrefillMax, kvd = (size_t)c.n_kv_heads * c.head_dim;
-    size_t nf = 0, nc = 0;
-    PrefillGroup g[4];
-    prefill_groups(m, m->layers[0], 1.0, g);  // every layer has the same shapes
-    for (auto& gr : g) {
-        size_t f, k;
-        prefill_scratch_need(gr, &f, &k);
-        nf = f > nf ? f : nf;
-        nc = k > nc ? k : nc;
-    }
+    size_t nf, nc;
+    row_scratch_need(m, &nf, &nc);
     int rc;
     if ((rc = model_alloc(m, m->pf_h, T * c.dim)) || (rc = model_alloc(m, m->pf_xn, T * c.dim)) ||
         (rc = model_alloc(m, m->pf_q, T * c.dim)) || (rc = model_alloc(m, m->pf_k, T * kvd)) ||
@@ -2166,6 +2182,330 @@ extern "C" int effort_model_prefill(effort_model_t* m, const int32_t* tokens_dev
         CK(cudaMemcpyAsync(m->pf_tok, tokens_dev + c0, sizeof(int32_t) * T, cudaMemcpyDeviceToDevice, s));
         m->host_pos += T;
         if ((rc = model_prefill_chunk(m, effort, T, s))) return rc;
+    }
+    return EFFORT_OK;
+}
+
+// ---- batch decode: up to kPrefillMax sequences per step, each with its own state (DESIGN.md section 4.9) -------------
+// A step is prefill's per-row path with one row per slot: embed, per layer rmsNorm*w rows -> [q,k,v] -> batch attention
+// (each slot on its own cache at its own position) -> wo into the residual rows -> rmsNorm*w -> [w1,w3] -> silu*mul -> w2
+// into the residual rows, then the final norm, the lm_head for every row, and each slot's tail as a model step ends it.
+struct effort_batch {
+    effort_model* m = nullptr;
+    int n = 0;                                 // slots
+    size_t slot_kv = 0;                        // floats of one slot's cache of one layer: max_seq * n_kv * 128
+    std::vector<float*> kc, vc;                // per layer: [n][max_seq][n_kv][128]
+    RowBuffers r{};                            // [n][...]
+    float* logits = nullptr;                   // [n + 1][vocab]: one row per slot, and a sink for the head's "last row" copy
+    float *part = nullptr, *cut = nullptr;     // multi-token GEMV scratch, owned: a batch never shares the model's
+    uint32_t* cnt = nullptr;
+    int *pos = nullptr, *tok = nullptr, *next = nullptr;  // [n]
+    std::vector<int> host_pos;                 // mirrors pos: bounds every slot's cache
+    std::vector<char> sampling;                // per slot: a sampler is set
+    bool sampler_dirty = false;
+    effort_sampler_t* sampler_dev = nullptr;   // [n], refreshed from the pinned sampler_host on the stream when it changed
+    effort_sampler_t* sampler_host = nullptr;
+    cudaEvent_t sampler_copied = nullptr;      // the last copy out of sampler_host has run
+    bool scoring = false;
+    int32_t* score_targets = nullptr;          // [n][max_seq], -1 = no target
+    effort_score_t* scores = nullptr;          // [n][max_seq]
+    bool warmed = false, stepped = false;
+    std::map<int, cudaGraphExec_t> graphs;     // keyed by q = Int(4095*(1-effort))
+    std::map<int, uint64_t> graph_launches;    // kernels one replay launches
+    std::vector<void*> owned;
+};
+
+template <typename T>
+static int batch_alloc(effort_batch* b, T*& p, size_t n) {
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); p = nullptr; return EFFORT_ENOMEM; }
+    CK(e);
+    b->owned.push_back(p);
+    CK(cudaMemset(p, 0, n * sizeof(T)));
+    return EFFORT_OK;
+}
+
+static void batch_drop_graphs(effort_batch* b) {
+    for (auto& g : b->graphs) cudaGraphExecDestroy(g.second);
+    b->graphs.clear();
+}
+
+static int batch_create_buffers(effort_batch* b) {
+    const auto& c = b->m->cfg;
+    const size_t N = b->n, kvd = (size_t)c.n_kv_heads * c.head_dim;
+    b->slot_kv = (size_t)c.max_seq * kvd;
+    b->kc.assign(c.n_layers, nullptr);
+    b->vc.assign(c.n_layers, nullptr);
+    int rc;
+    for (int li = 0; li < c.n_layers; li++)
+        if ((rc = batch_alloc(b, b->kc[li], N * b->slot_kv)) || (rc = batch_alloc(b, b->vc[li], N * b->slot_kv))) return rc;
+    size_t nf, nc;
+    row_scratch_need(b->m, &nf, &nc);
+    RowBuffers& r = b->r;
+    if ((rc = batch_alloc(b, r.h, N * c.dim)) || (rc = batch_alloc(b, r.xn, N * c.dim)) || (rc = batch_alloc(b, r.q, N * c.dim)) ||
+        (rc = batch_alloc(b, r.k, N * kvd)) || (rc = batch_alloc(b, r.v, N * kvd)) || (rc = batch_alloc(b, r.attn, N * c.dim)) ||
+        (rc = batch_alloc(b, r.x1, N * c.hidden_dim)) || (rc = batch_alloc(b, r.x3, N * c.hidden_dim)) ||
+        (rc = batch_alloc(b, r.x2, N * c.hidden_dim)) || (rc = batch_alloc(b, b->logits, (N + 1) * c.vocab)) ||
+        (rc = batch_alloc(b, b->part, nf)) || (rc = batch_alloc(b, b->cnt, nc)) ||
+        (rc = batch_alloc(b, b->cut, (size_t)kPrefillMax * kPrefillMaxProblems)) || (rc = batch_alloc(b, b->pos, N)) ||
+        (rc = batch_alloc(b, b->tok, N)) || (rc = batch_alloc(b, b->next, N)) || (rc = batch_alloc(b, b->sampler_dev, N)) ||
+        (rc = batch_alloc(b, b->score_targets, N * c.max_seq)) || (rc = batch_alloc(b, b->scores, N * c.max_seq)))
+        return rc;
+    CK(cudaMemset(b->score_targets, 0xff, sizeof(int32_t) * N * c.max_seq));  // all -1: no target
+    if (cudaMallocHost(&b->sampler_host, sizeof(effort_sampler_t) * N) != cudaSuccess) {
+        cudaGetLastError();
+        b->sampler_host = nullptr;
+        return EFFORT_ENOMEM;
+    }
+    CK(cudaEventCreateWithFlags(&b->sampler_copied, cudaEventDisableTiming));
+    b->host_pos.assign(N, 0);
+    b->sampling.assign(N, 0);
+    // kernel attributes before any capture
+    CK(cudaFuncSetAttribute(prefill_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)(kPrefillMax * c.dim * sizeof(__half))));
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_create(effort_model_t* m, int n_seq, effort_batch_t** out) {
+    if (!m || !out || n_seq < 1 || n_seq > kPrefillMax) return EFFORT_EINVAL;
+    *out = nullptr;
+    if (!model_prefill_fused(m)) return EFFORT_ESHAPE;
+    effort_batch* b = new (std::nothrow) effort_batch();
+    if (!b) return EFFORT_ENOMEM;
+    b->m = m;
+    b->n = n_seq;
+    const int rc = batch_create_buffers(b);
+    if (rc) {  // release what was allocated so far
+        effort_batch_destroy(b);
+        return rc;
+    }
+    *out = b;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_destroy(effort_batch_t* b) {
+    if (!b) return EFFORT_EINVAL;
+    batch_drop_graphs(b);
+    for (void* p : b->owned) cudaFree(p);
+    cudaFreeHost(b->sampler_host);
+    if (b->sampler_copied) cudaEventDestroy(b->sampler_copied);
+    delete b;
+    return EFFORT_OK;
+}
+
+// seq = -1: every slot
+static bool batch_slots(const effort_batch* b, int seq, int* s0, int* s1) {
+    if (seq < -1 || seq >= b->n) return false;
+    *s0 = seq < 0 ? 0 : seq;
+    *s1 = seq < 0 ? b->n : seq + 1;
+    return true;
+}
+
+extern "C" int effort_batch_reset(effort_batch_t* b, int seq, void* stream) {
+    int s0, s1;
+    if (!b || !batch_slots(b, seq, &s0, &s1)) return EFFORT_EINVAL;
+    CK(cudaMemsetAsync(b->pos + s0, 0, sizeof(int) * (s1 - s0), (cudaStream_t)stream));
+    for (int i = s0; i < s1; i++) b->host_pos[i] = 0;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_set_sampler(effort_batch_t* b, int seq, const effort_sampler_t* sp) {
+    int s0, s1;
+    if (!b || !batch_slots(b, seq, &s0, &s1) || (sp && !sampler_valid(sp))) return EFFORT_EINVAL;
+    CK(cudaEventSynchronize(b->sampler_copied));  // a copy still queued reads the pinned block
+    for (int i = s0; i < s1; i++) {
+        if (b->sampling[i] != (sp != nullptr)) batch_drop_graphs(b);  // the step's launch sequence changes
+        b->sampling[i] = sp != nullptr;
+        if (sp) {
+            b->sampler_host[i] = *sp;
+            b->sampler_dirty = true;
+        }
+    }
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_set_scoring(effort_batch_t* b, int enable) {
+    if (!b) return EFFORT_EINVAL;
+    if (b->scoring != (enable != 0)) batch_drop_graphs(b);
+    b->scoring = enable != 0;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_set_score_targets(effort_batch_t* b, int seq, const int32_t* targets_dev, int n, void* stream) {
+    int s0, s1;
+    if (!b || !batch_slots(b, seq, &s0, &s1)) return EFFORT_EINVAL;
+    const int max_seq = b->m->cfg.max_seq;
+    if (n < 0 || n > max_seq || (!targets_dev && n > 0)) return EFFORT_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    for (int i = s0; i < s1; i++) {
+        int32_t* row = b->score_targets + (size_t)i * max_seq;
+        if (n > 0) CK(cudaMemcpyAsync(row, targets_dev, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, s));
+        if (n < max_seq) CK(cudaMemsetAsync(row + n, 0xff, sizeof(int32_t) * (max_seq - n), s));
+    }
+    return EFFORT_OK;
+}
+
+extern "C" const float* effort_batch_logits(const effort_batch_t* b) { return b ? b->logits : nullptr; }
+extern "C" const int32_t* effort_batch_next_tokens(const effort_batch_t* b) { return b ? b->next : nullptr; }
+extern "C" const effort_score_t* effort_batch_scores(const effort_batch_t* b) { return b ? b->scores : nullptr; }
+
+extern "C" const void* effort_batch_buffer(const effort_batch_t* b, int which, int layer, int seq, size_t* count) {
+    if (count) *count = 0;
+    if (!b) return nullptr;
+    const auto& c = b->m->cfg;
+    const size_t N = b->n, kvd = (size_t)c.n_kv_heads * c.head_dim;
+    const void* p = nullptr;
+    size_t n = 0;
+    switch (which) {
+        case EFFORT_BUF_Q: if (b->stepped) { p = b->r.q; n = N * c.dim; } break;
+        case EFFORT_BUF_K: if (b->stepped) { p = b->r.k; n = N * kvd; } break;
+        case EFFORT_BUF_V: if (b->stepped) { p = b->r.v; n = N * kvd; } break;
+        case EFFORT_BUF_ATTN: if (b->stepped) { p = b->r.attn; n = N * c.dim; } break;
+        case EFFORT_BUF_KCACHE:
+        case EFFORT_BUF_VCACHE:
+            if (layer < 0 || layer >= c.n_layers || seq < 0 || seq >= b->n) return nullptr;
+            p = (which == EFFORT_BUF_KCACHE ? b->kc[layer] : b->vc[layer]) + (size_t)seq * b->slot_kv;
+            n = b->slot_kv;
+            break;
+        case EFFORT_BUF_POS: p = b->pos; n = N; break;
+        default: return nullptr;
+    }
+    if (p && count) *count = n;
+    return p;
+}
+
+static int batch_flush_sampler(effort_batch* b, cudaStream_t s) {
+    if (!b->sampler_dirty) return EFFORT_OK;
+    CK(cudaMemcpyAsync(b->sampler_dev, b->sampler_host, sizeof(effort_sampler_t) * b->n, cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(b->sampler_copied, s));
+    b->sampler_dirty = false;
+    return EFFORT_OK;
+}
+
+// what a model step ends with, for slot i on its logits row: the greedy argmax that advances the slot's position, the
+// slot's draw at that position, and with scoring on, record pos - 1 from the slot's target row
+static int batch_enqueue_tail(effort_batch* b, int i, cudaStream_t s) {
+    const auto& c = b->m->cfg;
+    const float* row = b->logits + (size_t)i * c.vocab;
+    CK(launch_pdl(argmax_advance_kernel, dim3(1), dim3(1024), 0, s, row, c.vocab, b->next + i, b->pos + i));
+    LAUNCHED();
+    int rc;
+    if (b->sampling[i] &&
+        (rc = enqueue_sample(b->m->ctx, row, c.vocab, b->sampler_host[i], b->sampler_dev + i, b->pos + i, 0u, b->next + i, s)))
+        return rc;
+    if (!b->scoring) return EFFORT_OK;
+    return enqueue_score(row, c.vocab, b->score_targets + (size_t)i * c.max_seq, c.max_seq, b->pos + i, 1,
+                         b->scores + (size_t)i * c.max_seq, s);
+}
+
+// one step of every slot, the tokens already in `tok` (no graph logic)
+static int batch_enqueue_step(effort_batch* b, double effort, cudaStream_t s) {
+    effort_model* m = b->m;
+    const auto& c = m->cfg;
+    effort_ctx* ctx = m->ctx;
+    const int T = b->n;
+    const RowBuffers& r = b->r;
+    int rc;
+    CK(launch_pdl(prefill_embed_kernel, dim3(T), dim3(256), 0, s, (const int*)b->tok, m->emb, c.dim, c.vocab, r.h));
+    LAUNCHED();
+    for (int li = 0; li < c.n_layers; li++) {
+        const auto& l = m->layers[li];
+        PrefillGroup g[4];
+        row_groups(ctx, l, effort, r, g);
+        for (auto& gr : g) gr.T = T;
+        CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)r.h, l.attn_norm, c.dim, c.norm_eps, r.xn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[0], b->part, b->cnt, b->cut, s))) return rc;
+        CK(launch_pdl(batch_attention_kernel, dim3(c.n_heads, T), dim3(256), 0, s, (const float*)r.q, (const float*)r.k,
+                      (const float*)r.v, b->kc[li], b->vc[li], b->slot_kv, (const int*)b->pos, c.n_heads, c.n_kv_heads,
+                      c.rope_theta, c.max_seq, r.attn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[1], b->part, b->cnt, b->cut, s))) return rc;
+        CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)r.h, l.ffn_norm, c.dim, c.norm_eps, r.xn));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[2], b->part, b->cnt, b->cut, s))) return rc;
+        const int nx = T * c.hidden_dim;
+        CK(launch_pdl(silu_mul_kernel, dim3((nx + 255) / 256), dim3(256), 0, s, (const float*)r.x1, (const float*)r.x3, nx, r.x2));
+        LAUNCHED();
+        if ((rc = enqueue_prefill_group(ctx, g[3], b->part, b->cnt, b->cut, s))) return rc;
+    }
+    CK(launch_pdl(prefill_rmsnorm_kernel, dim3(T), dim3(1024), 0, s, (const float*)r.h, m->norm, c.dim, c.norm_eps, r.xn));
+    LAUNCHED();
+    int grid = (c.vocab + 7) / 8;
+    if (grid > ctx->n_sms * 2) grid = ctx->n_sms * 2;
+    CK(launch_pdl(prefill_head_kernel, dim3(grid), dim3(256), (size_t)T * c.dim * sizeof(__half), s, (const float*)r.xn, T,
+                  m->out_core, c.vocab, c.dim, b->logits, b->logits + (size_t)T * c.vocab));
+    LAUNCHED();
+    for (int i = 0; i < T; i++)
+        if ((rc = batch_enqueue_tail(b, i, s))) return rc;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_step(effort_batch_t* b, const int32_t* tokens_dev, double effort, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (!b || !(effort >= 0.0 && effort <= 1.0)) return EFFORT_EINVAL;
+    effort_model* m = b->m;
+    if (!model_prefill_fused(m)) return EFFORT_ESHAPE;  // the chain or the context's options may have changed since create
+    for (int i = 0; i < b->n; i++)
+        if (b->host_pos[i] >= m->cfg.max_seq) return EFFORT_ESTATE;  // that slot's cache is full
+    CK(cudaMemcpyAsync(b->tok, tokens_dev ? (const void*)tokens_dev : (const void*)b->next, sizeof(int32_t) * b->n,
+                       cudaMemcpyDeviceToDevice, s));
+    for (int& p : b->host_pos) p++;
+    int rc;
+    if ((rc = batch_flush_sampler(b, s))) return rc;
+    b->stepped = true;
+    if (!m->use_graphs || s == nullptr) return batch_enqueue_step(b, effort, s);  // legacy stream cannot capture
+    const int key = effort_q(effort, EFFORT_PROBES_COUNT);
+    auto it = b->graphs.find(key);
+    if (it == b->graphs.end()) {
+        if (!b->warmed) {  // first step: eager (sets kernel attributes), as the model's first step
+            b->warmed = true;
+            return batch_enqueue_step(b, effort, s);
+        }
+        cudaGraph_t g = nullptr;
+        const uint64_t l0 = g_launches.load();
+        CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+        rc = batch_enqueue_step(b, effort, s);
+        cudaError_t e = cudaStreamEndCapture(s, &g);
+        if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+        CK(e);
+        cudaGraphExec_t ge = nullptr;
+        CK(cudaGraphInstantiate(&ge, g, 0));
+        CK(cudaGraphDestroy(g));
+        b->graphs[key] = ge;
+        b->graph_launches[key] = g_launches.load() - l0;
+        g_launches.store(l0);  // captured, not launched: the replay below counts them
+        it = b->graphs.find(key);
+    }
+    CK(cudaGraphLaunch(it->second, s));
+    g_launches.fetch_add(b->graph_launches[key]);
+    return EFFORT_OK;
+}
+
+extern "C" int effort_batch_fork(effort_batch_t* b, int seq, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    int s0, s1;
+    if (!b || !batch_slots(b, seq, &s0, &s1)) return EFFORT_EINVAL;
+    effort_model* m = b->m;
+    if (!model_prefill_fused(m)) return EFFORT_ESHAPE;
+    const int p = m->host_pos;
+    if (p == 0) return EFFORT_ESTATE;  // nothing to fork: no logits, no cache rows
+    const auto& c = m->cfg;
+    const size_t rows = (size_t)p * c.n_kv_heads * c.head_dim;
+    int rc;
+    if ((rc = batch_flush_sampler(b, s))) return rc;
+    for (int i = s0; i < s1; i++) {
+        for (int li = 0; li < c.n_layers; li++) {
+            CK(cudaMemcpyAsync(b->kc[li] + (size_t)i * b->slot_kv, m->layers[li].kc, sizeof(float) * rows, cudaMemcpyDeviceToDevice, s));
+            CK(cudaMemcpyAsync(b->vc[li] + (size_t)i * b->slot_kv, m->layers[li].vc, sizeof(float) * rows, cudaMemcpyDeviceToDevice, s));
+        }
+        CK(cudaMemcpyAsync(b->logits + (size_t)i * c.vocab, m->logits, sizeof(float) * c.vocab, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(b->pos + i, m->pos, sizeof(int), cudaMemcpyDeviceToDevice, s));
+        // the tail's argmax advances the position, as the head of the step that produced the logits did: start one back
+        CK(launch_pdl(prefill_advance_kernel, dim3(1), dim3(1), 0, s, b->pos + i, -1));
+        LAUNCHED();
+        if ((rc = batch_enqueue_tail(b, i, s))) return rc;
+        b->host_pos[i] = p;
     }
     return EFFORT_OK;
 }

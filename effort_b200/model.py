@@ -469,6 +469,71 @@ class DecodeModel:
         torch.cuda.current_stream().synchronize()
         return out.tolist()
 
+    def generate_batch(self, prompts: list[list[int]], n_new: int, effort: float = 0.25,
+                       samplers: Optional[list[Optional[dict]]] = None) -> list[list[int]]:
+        """Continue up to 16 prompts side by side (DESIGN.md section 4.9).  Each distinct prompt is prefilled into this model
+        once and forked into every slot that asks for it; then n_new - 1 batch steps on each slot's previous prediction.
+        samplers[b] is None (greedy) or set_sampler's keyword arguments for slot b.  Returns the n_new predicted tokens per
+        prompt.  The model is left at the last prompt; the host synchronises once, at the end."""
+        n = len(prompts)
+        if n < 1 or n_new < 1 or any(not p for p in prompts):
+            raise ValueError("generate_batch needs non-empty prompts and n_new >= 1")
+        longest = max(len(p) for p in prompts)
+        if longest + n_new - 1 > self.cfg.max_seq:
+            raise ValueError(f"prompt ({longest}) + n_new ({n_new}) - 1 positions exceed max_seq ({self.cfg.max_seq})")
+        batch = DecodeBatch(self, n)
+        for b, s in enumerate(samplers or []):
+            if s is not None:
+                batch.set_sampler(b, **s)
+        slots: dict[tuple, list[int]] = {}
+        for b, p in enumerate(prompts):
+            slots.setdefault(tuple(p), []).append(b)
+        for p, bs in slots.items():
+            self.reset()
+            self.prefill(list(p), effort)
+            for b in bs:
+                batch.fork(b)
+        out = torch.empty(n_new, n, dtype=torch.int32, device="cuda")
+        nxt = batch.next_tokens_view()
+        out[0].copy_(nxt)
+        for j in range(1, n_new):
+            batch.step(None, effort)
+            out[j].copy_(nxt)
+        rows = out.t().cpu()
+        return rows.tolist()
+
+    def score_continuations(self, context: list[int], continuations: list[list[int]],
+                            effort: float = 0.25) -> list[tuple[float, bool]]:
+        """Score up to 16 continuations of one context in lock step, HellaSwag style (DESIGN.md section 4.9): the context
+        is prefilled once and forked into one slot per continuation, whose tokens are teacher-forced; shorter continuations
+        are padded and their extra targets are -1.  Returns, per continuation, the summed log-probability of its tokens
+        and whether every one of them had rank 0 (was greedy's choice).  The host synchronises once."""
+        n, c = len(continuations), len(context)
+        if not context or n < 1 or any(not t for t in continuations):
+            raise ValueError("score_continuations needs a non-empty context and non-empty continuations")
+        L = max(len(t) for t in continuations)
+        if c + L - 1 > self.cfg.max_seq:
+            raise ValueError(f"context ({c}) + longest continuation ({L}) - 1 positions exceed max_seq ({self.cfg.max_seq})")
+        batch = DecodeBatch(self, n)
+        batch.set_scoring(True)
+        for b, t in enumerate(continuations):   # record c - 1 + j scores token j of the continuation
+            row = [-1] * (c - 1) + list(t) + [-1] * (L - len(t))
+            batch.set_score_targets(b, torch.tensor(row, dtype=torch.int32, device="cuda"))
+        feed = torch.tensor([[t[j] if j < len(t) else 0 for t in continuations] for j in range(L - 1)],
+                            dtype=torch.int32, device="cuda").view(max(L - 1, 0), n)
+        self.reset()
+        self.prefill(context, effort)
+        batch.fork()
+        for j in range(L - 1):
+            batch.step(feed[j], effort)
+        rank, logprob = batch.scores_view()[1:]
+        rank, logprob = rank.view(n, -1)[:, c - 1:c - 1 + L].cpu(), logprob.view(n, -1)[:, c - 1:c - 1 + L].cpu()
+        out = []
+        for b, t in enumerate(continuations):
+            k = len(t)
+            out.append((float(logprob[b, :k].double().sum()), bool((rank[b, :k] == 0).all())))
+        return out
+
     def logits(self) -> torch.Tensor:
         """Device logits of the last step as a torch view (copy)."""
         import numpy as np
@@ -510,6 +575,102 @@ class DecodeModel:
     @property
     def bucket_bytes(self) -> int:
         return int(self._L.effort_model_bucket_bytes(self._h))
+
+
+class DecodeBatch:
+    """Up to 16 sequences decoded together on one DecodeModel (effort_batch_*, DESIGN.md section 4.9).  Every slot has its
+    own KV caches, position, logits row, next token, sampler and score rows; a step feeds every slot one token.  A slot's
+    results do not depend on the batch size, its index or the other slots.  Keep the batch no longer than its model."""
+
+    def __init__(self, model: DecodeModel, n_seq: int):
+        self.model, self.cfg, self.n_seq = model, model.cfg, int(n_seq)
+        self._L = model._L
+        h = C.c_void_p()
+        check(self._L.effort_batch_create(model._h, self.n_seq, C.byref(h)), "effort_batch_create")
+        self._h = h
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                self._L.effort_batch_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    @staticmethod
+    def _seq(seq: Optional[int]) -> int:
+        return -1 if seq is None else int(seq)
+
+    def reset(self, seq: Optional[int] = None):
+        """Position 0 for slot `seq` (None = every slot)."""
+        check(self._L.effort_batch_reset(self._h, self._seq(seq), ops._stream_ptr()), "effort_batch_reset")
+
+    def fork(self, seq: Optional[int] = None):
+        """Copy the model's current state (cache rows, position, last logits) into slot `seq` (None = every slot) and end
+        it as a model step would: its greedy or sampled next token and, with scoring on, record pos - 1."""
+        check(self._L.effort_batch_fork(self._h, self._seq(seq), ops._stream_ptr()), "effort_batch_fork")
+
+    def step(self, tokens: Optional[torch.Tensor] = None, effort: float = 0.25):
+        """Enqueue one step of every slot (tokens: device int32 [n_seq]; None = each slot's previous prediction)."""
+        if tokens is not None:
+            ops._need(tokens, torch.int32, "tokens")
+            if tokens.numel() != self.n_seq:
+                raise ValueError(f"tokens must hold {self.n_seq} entries, got {tokens.numel()}")
+        check(self._L.effort_batch_step(self._h, None if tokens is None else tokens.data_ptr(), float(effort),
+                                        ops._stream_ptr()), "effort_batch_step")
+
+    def set_sampler(self, seq: Optional[int], temperature: Optional[float] = None, top_k: int = 0, top_p: float = 1.0,
+                    seed: int = 0):
+        """Slot `seq`'s sampler (None = every slot), as DecodeModel.set_sampler; temperature None = greedy."""
+        prm = None if temperature is None else _lib.Sampler(float(temperature), int(top_k), float(top_p), int(seed))
+        check(self._L.effort_batch_set_sampler(self._h, self._seq(seq), None if prm is None else C.byref(prm)),
+              "effort_batch_set_sampler")
+
+    def set_scoring(self, enable: bool):
+        check(self._L.effort_batch_set_scoring(self._h, 1 if enable else 0), "effort_batch_set_scoring")
+
+    def set_score_targets(self, seq: Optional[int], targets: Optional[torch.Tensor]):
+        """Slot `seq`'s targets (None = every slot), as DecodeModel.set_score_targets."""
+        n = 0 if targets is None else targets.numel()
+        if targets is not None:
+            ops._need(targets, torch.int32, "targets")
+        check(self._L.effort_batch_set_score_targets(self._h, self._seq(seq), None if targets is None else targets.data_ptr(),
+                                                     n, ops._stream_ptr()), "effort_batch_set_score_targets")
+
+    def scores_view(self) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """(argmax, rank, logprob) views of every slot's records, flat [n_seq * max_seq]"""
+        n = self.n_seq * self.cfg.max_seq
+        return ops.score_columns(_tensor_from_ptr(self._L.effort_batch_scores(self._h), 3 * n, torch.int32).view(n, 3))
+
+    def scores(self, seq: int) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """A device copy of slot `seq`'s records [max_seq] as (argmax, rank, logprob) columns."""
+        m = self.cfg.max_seq
+        return tuple(col[seq * m:(seq + 1) * m].clone() for col in self.scores_view())
+
+    def logits(self) -> torch.Tensor:
+        """A device copy of every slot's logits [n_seq][vocab]."""
+        return _tensor_from_ptr(self._L.effort_batch_logits(self._h), self.n_seq * self.cfg.vocab).view(self.n_seq, -1).clone()
+
+    def next_tokens_view(self) -> torch.Tensor:
+        return _tensor_from_ptr(self._L.effort_batch_next_tokens(self._h), self.n_seq, torch.int32)
+
+    def next_tokens(self) -> list[int]:
+        return self.next_tokens_view().cpu().tolist()
+
+    def buffer_view(self, name: str, layer: int = -1, seq: int = 0) -> Optional[torch.Tensor]:
+        """A flat device view of one of the batch's buffers (effort_batch_buffer): Q, K, V, ATTN as [n_seq][...] of the last
+        layer, KCACHE / VCACHE of `layer` (negative counts from the end) and slot `seq`, POS [n_seq]; None otherwise."""
+        if layer < 0:
+            layer += self.cfg.n_layers
+        n = C.c_size_t(0)
+        ptr = self._L.effort_batch_buffer(self._h, DecodeModel.BUFFERS[name], int(layer), int(seq), C.byref(n))
+        if not ptr:
+            return None
+        return _tensor_from_ptr(ptr, n.value, torch.int32 if name == "POS" else torch.float32)
+
+    def buffer(self, name: str, layer: int = -1, seq: int = 0) -> Optional[torch.Tensor]:
+        v = self.buffer_view(name, layer, seq)
+        return None if v is None else v.clone()
 
 
 class _CudaArray:

@@ -441,6 +441,50 @@ int effort_last_problem(effort_ctx_t* ctx, int slot, float* cutoff, uint32_t* n_
 int effort_bucket_mul_multi(effort_ctx_t* ctx, const float* v_dev, int n, const effort_weights_t* w, float* out_dev,
                             double effort, float* cutoff_dev, uint32_t* count_dev, void* stream);
 
+/*
+ * Batch decode (DESIGN.md section 4.9): n_seq (1..16) slots decoded together on one model, each with its own KV caches
+ * ([max_seq][n_kv][128] per layer), device position, logits row, next token, sampler (greedy by default) and score target
+ * and record rows ([max_seq] each).  A step feeds every slot one token and is prefill's per-row path with T = n_seq: the
+ * multi-token GEMV groups, an attention in which each slot reads its own cache at its own position, and one lm_head pass
+ * for all rows; each slot then ends as a model step does (greedy argmax advancing its position, its draw, its record
+ * pos - 1).  A slot's logits, next token, cache rows and records depend only on its own tokens, state, sampler
+ * parameters and the effort: not on n_seq, its index or the other slots.  The model's weights are read; the model's
+ * buffers are read only by fork.  Graphs follow effort_model_set_graphs: the first step runs eagerly, then one graph per
+ * effort is captured and replayed.  The batch's graphs hold the model's weight pointers: set the model's layers and head
+ * before creating a batch, and destroy the batch before its model.
+ */
+typedef struct effort_batch effort_batch_t;
+/* Allocates everything a step needs (caches, row buffers, GEMV scratch), so a captured graph never sees a reallocation.
+ * EFFORT_EINVAL for n_seq outside 1..16 or a NULL pointer; EFFORT_ESHAPE unless the model takes the multi-token prefill
+ * path (single GPU, chain 2, FP16 slice-major buckets, select cutoffs, no MoE); EFFORT_ENOMEM when the device is full. */
+int effort_batch_create(effort_model_t* m, int n_seq, effort_batch_t** out);
+int effort_batch_destroy(effort_batch_t* b);
+/* Every function below takes seq -1 for all slots where it takes a slot.  Reset: the slot's position becomes 0. */
+int effort_batch_reset(effort_batch_t* b, int seq, void* stream);
+/* Copies the model's current state into the slot (cache rows [0, pos) of every layer, the position and the last logits),
+ * then runs the slot's tail on those logits: greedy argmax, or a draw at position pos with the slot's sampler, and with
+ * scoring on, record pos - 1.  The slot is then where a model step would have left it.  Enqueue-only.  EFFORT_ESTATE
+ * (nothing enqueued) when the model is at position 0; EFFORT_ESHAPE as for create. */
+int effort_batch_fork(effort_batch_t* b, int seq, void* stream);
+/* One step of every slot: slot b takes tokens_dev[b] (device int32 [n_seq]), or its own previous next token when
+ * tokens_dev is NULL.  Enqueue-only.  EFFORT_EINVAL for effort outside [0, 1]; EFFORT_ESTATE (nothing enqueued) while any
+ * slot sits at max_seq; EFFORT_ESHAPE as for create. */
+int effort_batch_step(effort_batch_t* b, const int32_t* tokens_dev, double effort, void* stream);
+/* The slot's sampler, as effort_model_set_sampler: NULL = greedy.  Parameters are copied on the stream of the next step
+ * or fork, without recapture; switching a slot between greedy and sampling drops the batch's graphs. */
+int effort_batch_set_sampler(effort_batch_t* b, int seq, const effort_sampler_t* s);
+/* Off by default; switching drops the batch's graphs.  As effort_model_set_scoring, per slot. */
+int effort_batch_set_scoring(effort_batch_t* b, int enable);
+/* As effort_model_set_score_targets, into the slot's target row. */
+int effort_batch_set_score_targets(effort_batch_t* b, int seq, const int32_t* targets_dev, int n, void* stream);
+const float* effort_batch_logits(const effort_batch_t* b);          /* device [n_seq][vocab] */
+const int32_t* effort_batch_next_tokens(const effort_batch_t* b);   /* device [n_seq] */
+const effort_score_t* effort_batch_scores(const effort_batch_t* b); /* device [n_seq][max_seq] */
+/* Test hook, as effort_model_buffer: EFFORT_BUF_Q / K / V / ATTN give the last layer's values of the last step as
+ * [n_seq][...] (NULL before the first step); KCACHE / VCACHE give `layer`'s cache of slot `seq`; POS gives [n_seq]; every
+ * other id gives NULL. */
+const void* effort_batch_buffer(const effort_batch_t* b, int which, int layer, int seq, size_t* count);
+
 /* ---- introspection used by bench / tests -------------------------------- */
 /* number of kernels this library has launched since load (process-wide) */
 uint64_t effort_launch_count(void);
