@@ -38,6 +38,8 @@ SIGNATURES = {
                                         C.c_uint, vp, C.POINTER(C.c_void_p)]),
     "effort_weights_destroy": (C.c_int, [C.c_void_p]),
     "effort_weights_owned_bytes": (C.c_size_t, [C.c_void_p]),
+    "effort_weights_hint": (C.c_void_p, [C.c_void_p]),
+    "effort_pdl_enabled": (C.c_int, []),
     "effort_bucket_mul": (C.c_int, [vp, fp, vp, u32p, fp, C.c_double, vp]),
     "effort_bucket_mul_q4": (C.c_int, [vp, fp, vp, u32p, fp, C.c_double, vp]),
     "effort_expert_mul": (C.c_int, [vp, fp, vp, u32p, fp, C.c_double, vp]),
@@ -65,6 +67,7 @@ SIGNATURES = {
     "effort_model_set_moe": (C.c_int, [vp, C.c_int, vp, C.c_int]),
     "effort_model_set_head": (C.c_int, [vp, vp, vp, vp]),
     "effort_model_reset": (C.c_int, [vp, vp]),
+    "effort_model_rewind": (C.c_int, [vp, C.c_int, vp]),
     "effort_model_step": (C.c_int, [vp, vp, C.c_double, vp]),
     "effort_model_prefill": (C.c_int, [vp, vp, C.c_int, C.c_double, vp]),
     "effort_bucket_mul_multi": (C.c_int, [vp, vp, C.c_int, vp, vp, C.c_double, vp, vp, vp]),

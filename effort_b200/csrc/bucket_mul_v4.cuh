@@ -43,6 +43,7 @@ struct V4Header {
     uint2 sel_slot[2][kV4SelWarps];      // select mode: per-warp packed counts, double buffered by round parity
     float red[kV4SelWarps];
     float cutoff, denom;
+    float hint;                          // the matrix's cutoff hint as thread 0 read it: one value for the whole select group
     int sel_rows;
     uint32_t warp_rows[kV2Threads / 32]; // rows selected by each warp's records (the split below)
     uint32_t start[kV4Pairs + 1];        // start[q]: the record holding pair q's first row (start[kV4Pairs] = records)
@@ -131,7 +132,7 @@ __device__ __forceinline__ uint32_t count_gt32(const uint32_t (&keys)[kSelKeys],
 // Q(R) false and evaluates three interior thresholds per round (one pass over the keys, one 128-thread barrier).  Eight
 // rounds from scratch.  With a hint -- the key of the cutoff this matrix saw on the previous call -- the first round
 // brackets it (hint +- 16 keys = +- 12 % in value) and two more rounds finish when the guess holds; a miss only costs the
-// bracketing round.  The result does not depend on the hint.
+// bracketing round.  The result does not depend on the hint, provided every thread of the group passes the same one.
 __device__ __forceinline__ float select_cutoff_group(const uint32_t (&keys)[kSelKeys], int k, V4Header& hdr, int gt, uint32_t hint_key,
                                                      int* rounds_out) {
     const int lane = gt & 31, gw = gt >> 5;
@@ -328,6 +329,7 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
     }
     if constexpr (CUT == kCutSelect) {
         if (sel_warp) {
+            if (tid == 0 && pb.cutoff_hint) hdr.hint = pb.cutoff_hint[e_no];  // published by the barrier before the select
             const float* src = (vmode == kVPlain) ? pb.v_cut : pb.v;
             float vv[kSelVals];
 #pragma unroll
@@ -380,7 +382,13 @@ bucket_mul_v4_kernel(const __grid_constant__ V2Batch batch) {
             if (cst) cst[2] = (unsigned long long)clock64();
             uint32_t hint_key = 0u;
             if (pb.cutoff_hint) {  // last cutoff of this matrix (kVNorm: stored times that call's denominator)
-                const float hc = pb.cutoff_hint[e_no] / denom;
+                // Every select warp must start from the SAME hint.  CTA 0 of this launch overwrites it once its cutoff is
+                // known, and warps that each loaded it could fall on either side of that store: they would then probe
+                // different thresholds in the same round, sum counts that belong to no single threshold, and settle on a
+                // wrong cutoff for this CTA (a bit-level divergence that only timing triggers, DESIGN.md section 4.7).
+                // kVNorm: the denominator's barrier above already published hdr.hint.
+                if (vmode != kVNorm) asm volatile("bar.sync 2, %0;" ::"n"(kV4SelWarps * 32) : "memory");
+                const float hc = hdr.hint / denom;
                 hint_key = (hc > 0.f && hc < 3e38f) ? (__float_as_uint(hc) >> 16) : 0u;
             }
             const float cut = select_cutoff_group(keys, EFFORT_PROBES_MAX - pb.q, hdr, tid, hint_key,

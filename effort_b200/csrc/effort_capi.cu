@@ -245,6 +245,7 @@ static bool pdl_enabled() {
     if (v < 0) { const char* e = getenv("EFFORT_PDL"); v = (e && atoi(e) == 0) ? 0 : 1; }
     return v == 1;
 }
+extern "C" int effort_pdl_enabled(void) { return pdl_enabled() ? 1 : 0; }
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
                               Args&&... args) {
@@ -356,6 +357,7 @@ extern "C" int effort_weights_destroy(effort_weights_t* w) {
     return EFFORT_OK;
 }
 extern "C" size_t effort_weights_owned_bytes(const effort_weights_t* w) { return w ? w->owned : 0; }
+extern "C" float* effort_weights_hint(const effort_weights_t* w) { return w ? w->hint : nullptr; }
 
 // ---------------------------------------------------------------------------------------------------
 // helpers
@@ -1495,6 +1497,14 @@ extern "C" int effort_model_reset(effort_model_t* m, void* stream) {
     if (!m) return EFFORT_EINVAL;
     CK(cudaMemsetAsync(m->pos, 0, sizeof(int), (cudaStream_t)stream));
     m->host_pos = 0;
+    return EFFORT_OK;
+}
+
+extern "C" int effort_model_rewind(effort_model_t* m, int pos, void* stream) {
+    if (!m || pos < 0 || pos >= m->cfg.max_seq) return EFFORT_EINVAL;
+    // pageable source: the copy has taken the value once the call returns
+    CK(cudaMemcpyAsync(m->pos, &pos, sizeof(int), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    m->host_pos = pos;
     return EFFORT_OK;
 }
 

@@ -341,6 +341,11 @@ class DecodeModel:
     def reset(self):
         check(self._L.effort_model_reset(self._h, ops._stream_ptr()), "effort_model_reset")
 
+    def rewind(self, pos: int):
+        """Set the position to `pos` (0 <= pos < max_seq), keeping the cache rows: the next step repeats step `pos` on
+        the rows the earlier steps left (a test hook for repeating one step from a fixed state)."""
+        check(self._L.effort_model_rewind(self._h, int(pos), ops._stream_ptr()), "effort_model_rewind")
+
     def set_graphs(self, enable: bool):
         check(self._L.effort_model_set_graphs(self._h, 1 if enable else 0), "effort_model_set_graphs")
 

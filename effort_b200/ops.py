@@ -140,6 +140,14 @@ class ExpertWeights:
     def owned_bytes(self) -> int:
         return int(self._L.effort_weights_owned_bytes(self._h))
 
+    def hint(self) -> Optional[torch.Tensor]:
+        """A live device view of the matrix's cutoff hints [n_experts] (effort_weights_hint, a test hook), or None."""
+        ptr = self._L.effort_weights_hint(self._h)
+        if not ptr:
+            return None
+        from .model import _tensor_from_ptr
+        return _tensor_from_ptr(ptr, self.numExperts)
+
     def __del__(self):
         try:
             if getattr(self, "_h", None):
@@ -343,6 +351,11 @@ def score(logits: torch.Tensor, targets: torch.Tensor, ctx: Optional[Context] = 
     check(ctx._L.effort_score(ctx._h, logits.data_ptr(), logits.numel(), targets.data_ptr(), targets.numel(), rec.data_ptr(),
                               _stream_ptr()), "score")
     return score_columns(rec)
+
+
+def pdl_enabled() -> bool:
+    """whether kernels are launched with programmatic dependent launch (EFFORT_PDL, read once per process)"""
+    return bool(_lib.load().effort_pdl_enabled())
 
 
 def launchCount() -> int:

@@ -124,6 +124,12 @@ int effort_weights_create(const void* buckets_dev, const void* stats_dev, const 
 int effort_weights_destroy(effort_weights_t* w);
 /* bytes of device memory the handle owns (the repacked copy) */
 size_t effort_weights_owned_bytes(const effort_weights_t* w);
+/* Test hooks.  The matrix's cutoff hints, device float [n_experts] (the last cutoff each expert's select found, times
+ * the rmsNorm denominator on norm-on-load launches; +inf before the first; NULL for weights the default kernel does not
+ * run), which a caller may overwrite between launches: the select's result does not depend on them.  And whether
+ * kernels are launched with programmatic dependent launch (EFFORT_PDL, read once per process). */
+float* effort_weights_hint(const effort_weights_t* w);
+int effort_pdl_enabled(void);
 
 /* ---- the operator ------------------------------------------------------ */
 /*
@@ -271,6 +277,9 @@ int effort_model_set_head(effort_model_t* m, const void* norm_dev, const void* o
                           const void* tok_embeddings_dev);
 /* position <- 0 (the KV cache is logically emptied) */
 int effort_model_reset(effort_model_t* m, void* stream);
+/* position <- pos, 0 <= pos < max_seq (a test hook): the cache rows stay, as after a reset, so the next step repeats
+ * step pos on the rows the earlier steps left.  EINVAL for a NULL model or pos out of range. */
+int effort_model_rewind(effort_model_t* m, int pos, void* stream);
 /*
  * One decode step at the current position, enqueue-only.  token_dev: device int32 (NULL = the token the
  * previous step predicted).  After it: logits in effort_model_logits(), next token in effort_model_next_token().

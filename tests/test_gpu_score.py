@@ -238,9 +238,8 @@ def test_with_a_sampler(small_model):
 
 def test_score_every_position_up_to_max_seq():
     """score() at every position up to max_seq, each record checked at 33 positions against the model on that step's
-    logits.  Byte-identical repeats are checked over the first 1024 positions: on the H100, 7 of 16 scoring-on runs of
-    this 2048-token decode diverged from the scoring-off decode at one layer-1 K/V cache row between positions 1197 and
-    1752 (DESIGN.md section 4.7), and none below."""
+    logits, and two more score() runs over all max_seq positions byte-identical to each other and to the step-by-step
+    records."""
     import torch
     from effort_b200.model import DecodeModel, MistralConfig
     cfg = MistralConfig(n_layers=2, vocab=32000, max_seq=2048)
@@ -269,8 +268,8 @@ def test_score_every_position_up_to_max_seq():
     a, r, l = m.scores()
     assert int(r[2047]) == -1 and torch.isnan(l[2047])
     print(f"score(): 2048 positions, max |logprob - float64| / bar at 33 of them = {worst:.3f}")
-    # the first 1024 positions: two score() runs and the step-by-step records agree byte for byte
-    n = 1024
+    # every position: two score() runs and the step-by-step records agree byte for byte
+    n = cfg.max_seq
     p1, l1, r1 = m.score(seq[:n], 0.25)
     p2, l2, r2 = m.score(seq[:n], 0.25)
     assert torch.equal(p1, p2) and torch.equal(r1, r2) and torch.equal(l1.view(torch.int32), l2.view(torch.int32))
